@@ -569,7 +569,7 @@ attn_decode_item_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_c
 // =================================================================================
 // prefill (causal, chunk-capable: queries may start at any position of the sequence)
 // =================================================================================
-// Round 1's mma.sync prefill kernel: kept ONLY as the A/B baseline of the tcgen05 kernel
+// Round 1's mma.sync prefill kernel: kept ONLY as the A/B baseline of the wgmma kernel
 // (attention_prefill_tc.cu; ACP_ATTN_PREFILL_TC=0 and tests/test_attention_gpu.py impl 0).
 constexpr int NS = STAGES;
 __global__ void __launch_bounds__(ATTN_THREADS, 2)

@@ -57,7 +57,7 @@ size_t attn_decode_ws_floats(int max_batch, int heads, int kv_heads, int max_chu
 int launch_attn_decode(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const AttnDecodeArgs& a,
                        cudaStream_t s);
 int attn_prefill_block_tokens(int heads, int kv_heads);
-// tcgen05 prefill attention (attention_prefill_tc.cu): 128 query rows = 128/G tokens x G heads per CTA
+// wgmma prefill attention (attention_prefill_tc.cu): 128 query rows = 128/G tokens x G heads per CTA
 int attn_prefill_tc_setup();
 int attn_prefill_tc_block_tokens(int heads, int kv_heads);
 int attn_make_kv_half_map(CUtensorMap* out, const void* base, uint64_t num_pages, int kv_heads);

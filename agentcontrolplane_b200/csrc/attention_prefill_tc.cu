@@ -1,5 +1,5 @@
-// attention_prefill_tc.cu — causal paged-KV GQA attention for PREFILL steps on the 5th-gen tensor
-// cores: S = Q K^T and O += P V are tcgen05.mma with the accumulators in TMEM.
+// attention_prefill_tc.cu — causal paged-KV GQA attention for PREFILL steps on the Hopper tensor
+// cores: S = Q K^T and O += P V are wgmma warpgroup MMAs with the accumulators in registers.
 //
 // CTA = 128 query rows x one KV head.  GQA packs the G = heads / kv_heads query heads that share
 // the KV head into the rows: row r = (token r / G, head r % G), i.e. 128 / G consecutive new tokens
@@ -8,23 +8,19 @@
 // boundaries are ABSOLUTE key indices, so a row's arithmetic depends only on its own sequence
 // (chunked prefill == single shot, batch invariance).
 //
-//   warp 0     TMA producer: Q tile once (3-D map over qbuf [T][heads][128], box {64, G, 128/G}),
-//              then per tile K and V as four {64 dims x 32 tokens} boxes each (page x dim-half),
-//              two 2-deep rings with their own full/empty mbarriers
-//   warp 1     TMEM alloc (256 columns) + single-thread MMA issuer:
-//                S[b]  = Q K_j^T   M=128 N=64  K=128  (A, B from smem, both K-major, SW128)
-//                O    += P_j V_j   M=128 N=128 K=64   (A = P from TMEM, B = V from smem MN-major)
-//              S is double-buffered in TMEM (columns 0..63 / 64..127): QK_{j+1} is issued before
-//              PV_j, so the tensor pipe works on the next tile while the softmax warps are busy.
-//   warps 2-5  softmax: thread = one row (TMEM lane).  tcgen05.ld the 64 scores, causal mask on
-//              diagonal tiles, running max with LAZY rescale (O and l are only rescaled when the max
-//              grows by more than 2^8; exact, the normaliser carries the same stale max), exp2,
-//              P = bf16 hi + bf16 lo (two PV MMAs ~ fp32 P, so no P rounding has to be mirrored by
-//              the oracle — same policy as the decode kernels), tcgen05.st P over the S columns it
-//              just read, O rescale via tcgen05.ld/st when needed, final O / l -> bf16 -> global.
-// Two CTAs per SM (96 KiB smem, 256 TMEM columns each): one CTA's MMAs overlap the other's softmax.
+//   warpgroups 0, 1  rows 0..63 / 64..127.  Per tile:
+//                S  = Q K_j^T  m64n64k16 x 8   (A = Q, B = K, both from smem, K-major, SW128)
+//                softmax in registers (a thread owns 2 rows x 16 keys; row max / sum over the 4-lane quad):
+//                causal mask on diagonal tiles, running max with LAZY rescale (O and l are only rescaled
+//                when the max grows by more than 2^8; exact, the normaliser carries the same stale max),
+//                exp2, P = bf16 hi + bf16 lo (two PV MMAs ~ fp32 P, so no P rounding has to be mirrored
+//                by the oracle — same policy as the decode kernels)
+//                O += P V_j    m64n128k16 x 4 x 2 (A = P from registers, B = V from smem, MN-major)
+//   warp 8      TMA producer: Q tile once (3-D map over qbuf [T][heads][128], box {64, G, 128/G}),
+//               then per tile K and V as four {64 dims x 32 tokens} boxes each (page x dim-half),
+//               two 2-deep rings with their own full/empty mbarriers
+// The two warpgroups interleave on the SM: one's MMAs overlap the other's softmax.
 //
-// Replaces round 1's mma.sync prefill kernel (116 TFLOP/s, profiles/r1_v2_ncu_prefill_kernels.md).
 // Reference boundary: part of the arithmetic behind langchaingo_client.go:102 (DESIGN.md §1).
 #include "attention.h"
 #include "common.cuh"
@@ -41,37 +37,9 @@ constexpr int PF_Q_BYTES = 2 * PF_ROWS * 128;    // 2 k-blocks (64 dims) of [128
 constexpr int PF_KT_BYTES = 2 * PF_KEYS * 128;   // 2 dim-halves of [64 keys][128 B] = 16 KiB
 constexpr int PF_HALF_BYTES = PF_KEYS * 128;     // 8 KiB
 constexpr int PF_PAGE_BYTES = KV_PAGE * 128;     // one {64 x 32} box = 4 KiB
-constexpr int PF_THREADS = 192;
+constexpr int PF_THREADS = 288;                  // 2 consumer warpgroups + 1 producer warp
 constexpr int PF_SMEM = 1024 + PF_Q_BYTES + 2 * PF_STAGES * PF_KT_BYTES + 256;
-constexpr uint32_t PF_TMEM_COLS = 256;
-constexpr uint32_t PF_COL_S0 = 0, PF_COL_O = 128;   // S[b] at columns b*64, O at 128..255
-constexpr float PF_RESCALE_LOG2 = 8.0f;             // lazy rescale threshold (log2 units)
-
-ACP_DEVINL void tmem_ld_x32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-ACP_DEVINL void tmem_st_x32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      :
-      : "r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]),
-        "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]),
-        "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-ACP_DEVINL void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+constexpr float PF_RESCALE_LOG2 = 8.0f;          // lazy rescale threshold (log2 units)
 
 // two fp32 -> packed bf16x2 (round to nearest even) in ONE conversion instruction; `lo` lands in bits 0..15
 ACP_DEVINL uint32_t cvt_bf16x2(float lo, float hi) {
@@ -91,31 +59,6 @@ ACP_DEVINL void split_hi_lo(float p0, float p1, uint32_t& hi, uint32_t& lo) {
   lo = cvt_bf16x2(p0 - __uint_as_float(hi << 16), p1 - __uint_as_float(hi & 0xffff0000u));
 }
 
-// D[tmem] (+)= A[tmem, bf16 pairs per 32-bit column] * B[smem desc]
-ACP_DEVINL void umma_bf16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      :
-      : "r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-
-// UMMA shared-memory descriptor of an MN-major operand, SWIZZLE_128B (canonical layout, in 16-byte
-// units: ((8,n),(8,k)) : ((1,LBO),(8,SBO)) — cute/atom/mma_traits_sm100.hpp): a row of 128 B runs
-// along MN (64 bf16), 8 rows along K form the 1024-B swizzle atom, SBO = distance between 8-row
-// K groups, LBO = distance between 64-element MN atoms.
-ACP_DEVINL uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= (uint64_t)((smem_addr & 0x3ffffu) >> 4);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3fffu) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3fffu) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)2 << 61;
-  return d;
-}
-
 ACP_DEVINL void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, uint64_t hint) {
   asm volatile(
       "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint"
@@ -128,12 +71,9 @@ ACP_DEVINL void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int
 struct PfBars {
   uint64_t q_full;
   uint64_t k_full[PF_STAGES], k_empty[PF_STAGES], v_full[PF_STAGES], v_empty[PF_STAGES];
-  uint64_t s_full[2], p_full[2];
-  uint64_t pv_done;
-  uint32_t tmem_slot;
 };
 
-__global__ void __launch_bounds__(PF_THREADS, 2)
+__global__ void __launch_bounds__(PF_THREADS, 1)
 attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_constant__ CUtensorMap tm_k,
                        const __grid_constant__ CUtensorMap tm_v, AttnPrefillArgs a, int num_blocks) {
   extern __shared__ uint8_t smem_raw[];
@@ -163,20 +103,14 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     tma_prefetch_desc(&tm_v);
     mbar_init(&bars->q_full, 1);
     for (int s = 0; s < PF_STAGES; ++s) {
-      mbar_init(&bars->k_full[s], 1); mbar_init(&bars->k_empty[s], 1);
-      mbar_init(&bars->v_full[s], 1); mbar_init(&bars->v_empty[s], 1);
+      mbar_init(&bars->k_full[s], 1); mbar_init(&bars->k_empty[s], 8);
+      mbar_init(&bars->v_full[s], 1); mbar_init(&bars->v_empty[s], 8);
     }
-    for (int s = 0; s < 2; ++s) { mbar_init(&bars->s_full[s], 1); mbar_init(&bars->p_full[s], 4); }
-    mbar_init(&bars->pv_done, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc(&bars->tmem_slot, PF_TMEM_COLS);
-  tcgen05_fence_before();
   __syncthreads();
-  tcgen05_fence_after();
-  const uint32_t tmem_base = bars->tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ===================== TMA producer =====================
     if (lane == 0) {
       pdl_wait();   // q and the K/V pages of this step come from the previous kernel (rope_kv)
@@ -186,7 +120,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
       tma_load_3d(q_smem + PF_ROWS * 128, &tm_q, &bars->q_full, 64, kh * G, row0, kEvictFirst);
       const int* pt_row = a.page_table + (size_t)b * a.max_pages;
       int jk = 0, jv = 0;
-      uint32_t spins = 0;
+      uint64_t t0 = 0;
       while (jv < n_tiles) {
         bool progressed = false;
         // K runs up to two tiles ahead of the MMAs, V follows K; neither blocks the other
@@ -218,193 +152,126 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
           ++jv;
           progressed = true;
         }
-        if (progressed) spins = 0;
-        else if (++spins > (1u << 26)) {
-          printf("[acp_infer] attn_prefill_tc producer timeout block=(%d,%d) jk=%d jv=%d\n", blockIdx.x, blockIdx.y, jk, jv);
-          __trap();
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer =====================
-    if (lane == 0) {
-      constexpr uint32_t idesc_qk = umma_idesc_bf16(PF_ROWS, PF_KEYS);                 // A, B K-major
-      constexpr uint32_t idesc_pv = umma_idesc_bf16(PF_ROWS, HEAD_DIM) | (1u << 16);   // B (= V) MN-major
-      const uint32_t q_addr = smem_u32(q_smem);
-      auto issue_qk = [&](int j) {
-        const int s = j % PF_STAGES;
-        mbar_wait(&bars->k_full[s], ((uint32_t)(j / PF_STAGES)) & 1u);
-        tcgen05_fence_after();
-        const uint32_t k_addr = smem_u32(k_smem + s * PF_KT_BYTES);
-        const uint32_t d = tmem_base + PF_COL_S0 + (uint32_t)(j & 1) * PF_KEYS;
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {     // dim halves = 64-wide k-blocks
-          const uint64_t a_desc = umma_desc_k_sw128(q_addr + h * (PF_ROWS * 128));
-          const uint64_t b_desc = umma_desc_k_sw128(k_addr + h * PF_HALF_BYTES);
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_bf16(d, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), idesc_qk, (h | k) ? 1u : 0u);
-        }
-        umma_commit(&bars->k_empty[s]);
-        umma_commit(&bars->s_full[j & 1]);
-      };
-      mbar_wait(&bars->q_full, 0);
-      tcgen05_fence_after();
-      issue_qk(0);
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) issue_qk(j + 1);
-        mbar_wait(&bars->p_full[j & 1], ((uint32_t)(j >> 1)) & 1u);   // P_j written, O rescaled
-        const int s = j % PF_STAGES;
-        mbar_wait(&bars->v_full[s], ((uint32_t)(j / PF_STAGES)) & 1u);
-        tcgen05_fence_after();
-        const uint32_t v_addr = smem_u32(v_smem + s * PF_KT_BYTES);
-        const uint32_t p_addr = tmem_base + PF_COL_S0 + (uint32_t)(j & 1) * PF_KEYS;   // hi at +0, lo at +32
-        const uint32_t o_addr = tmem_base + PF_COL_O;
-#pragma unroll
-        for (int part = 0; part < 2; ++part) {       // P hi, then P lo
-#pragma unroll
-          for (int kk = 0; kk < PF_KEYS / 16; ++kk) {   // 16 keys per MMA: 8 TMEM columns of packed bf16 pairs
-            const uint64_t b_desc = umma_desc_mn_sw128(v_addr + kk * 16 * 128, PF_HALF_BYTES, 1024);
-            umma_bf16_ts(o_addr, p_addr + (uint32_t)(part * 32 + kk * 8), b_desc, idesc_pv, (j | part | kk) ? 1u : 0u);
-          }
-        }
-        umma_commit(&bars->v_empty[s]);
-        umma_commit(&bars->pv_done);
+        // the bound of mbar_wait_mma (no printf: it would serialize the kernel's wgmma)
+        if (progressed) t0 = 0;
+        else if (t0 == 0) t0 = global_timer_ns();
+        else if (global_timer_ns() - t0 > 20000000000ull) __trap();
       }
     }
   } else {
-    // ===================== softmax warps 2..5: thread = one query row =====================
-    const int q = warp & 3;                        // TMEM lane quarter this warp may access
-    const int r = q * 32 + lane;                   // row of the tile = TMEM lane
-    const int t = r / G, g = r % G;
-    const int tq = tq0 + t;
-    const bool valid = t < blk_tokens;
-    const int limit = valid ? pos0 + tq + 1 : 0;   // keys with index < limit are visible
+    // ============ consumer warpgroups: thread owns rows rb and rb + 8, keys 8c + 2(lane % 4) + {0, 1} ============
+    const int wg = warp >> 2;
+    const int rb = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    int limit[2], tok[2], head[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int r = rb + 8 * h;
+      tok[h] = r / G;
+      head[h] = r % G;
+      limit[h] = tok[h] < blk_tokens ? pos0 + tq0 + tok[h] + 1 : 0;   // keys with index < limit are visible
+    }
     const int first_limit = pos0 + tq0 + 1;        // smallest limit among the valid rows of this CTA
     const float sl2e = a.scale * 1.4426950408889634f;
-    const uint32_t lane_base = (uint32_t)(q * 32) << 16;
     pdl_wait();
-    float m_run = -INFINITY;   // running max, log2 units (score * sl2e); stale by at most PF_RESCALE_LOG2
-    float l_run = 0.f;
+    float m_run[2] = {-INFINITY, -INFINITY};   // running max, log2 units (score * sl2e); stale by at most PF_RESCALE_LOG2
+    float l_run[2] = {0.f, 0.f};               // this thread's share of the row sums
+    float o[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] = 0.f;
+    const uint32_t q_addr = smem_u32(q_smem) + (uint32_t)wg * (64 * 128);
+    mbar_wait_mma(&bars->q_full, 0);
     for (int j = 0; j < n_tiles; ++j) {
-      const int bsel = j & 1;
-      mbar_wait(&bars->s_full[bsel], ((uint32_t)(j >> 1)) & 1u);
-      tcgen05_fence_after();
-      const uint32_t s_addr = tmem_base + lane_base + PF_COL_S0 + (uint32_t)bsel * PF_KEYS;
-      uint32_t sr0[32], sr1[32];
-      tmem_ld_x32(s_addr, sr0);
-      tmem_ld_x32(s_addr + 32, sr1);
-      tmem_ld_wait();
+      const int s = j % PF_STAGES;
+      const uint32_t par = ((uint32_t)(j / PF_STAGES)) & 1u;
+      float sc[32];
+      mbar_wait_mma(&bars->k_full[s], par);
+      {
+        const uint32_t k_addr = smem_u32(k_smem + s * PF_KT_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {     // dim halves = 64-wide k-blocks
+          const uint64_t a_desc = gmma_desc_k_sw128(q_addr + h * (PF_ROWS * 128));
+          const uint64_t b_desc = gmma_desc_k_sw128(k_addr + h * PF_HALF_BYTES);
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            wgmma_bf16_ss<PF_KEYS>(sc, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), (h | k) ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(sc);
+      }
+      if (lane == 0) mbar_arrive(&bars->k_empty[s]);
       const int tile0 = j * PF_KEYS;
-      float mx = -INFINITY;
       if (tile0 + PF_KEYS > first_limit) {   // diagonal tile: causal mask (CTA-uniform branch)
 #pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          if (tile0 + c >= limit) sr0[c] = 0xff800000u;        // -inf
-          if (tile0 + 32 + c >= limit) sr1[c] = 0xff800000u;
+        for (int i = 0; i < 32; ++i)
+          if (tile0 + 8 * (i >> 2) + 2 * (lane & 3) + (i & 1) >= limit[(i >> 1) & 1]) sc[i] = -INFINITY;
+      }
+      float base[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float mx = -INFINITY;
+#pragma unroll
+        for (int c = 0; c < 8; ++c) mx = fmaxf(mx, fmaxf(sc[4 * c + 2 * h], sc[4 * c + 2 * h + 1]));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float cand = mx * sl2e;
+        // lazy rescale: keep the old base unless the max grew by more than 2^8 (or there was none)
+        if (m_run[h] == -INFINITY) {
+          m_run[h] = cand;                   // first visible key of this row (O and l are still 0)
+        } else if (cand > m_run[h] + PF_RESCALE_LOG2) {
+          const float corr = ex2_ftz(m_run[h] - cand);
+          m_run[h] = cand;
+          l_run[h] *= corr;
+#pragma unroll
+          for (int c = 0; c < 16; ++c) { o[4 * c + 2 * h] *= corr; o[4 * c + 2 * h + 1] *= corr; }
         }
+        base[h] = (m_run[h] == -INFINITY) ? 0.f : m_run[h];
       }
-      {  // four independent max chains (a single one is 32 dependent FMNMX)
-        float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
+      // P as the A fragments of four k16 MMAs: keys 16kk..16kk+15 = score registers 8kk..8kk+7
+      uint32_t ph[16], pl[16];
 #pragma unroll
-        for (int c = 0; c < 32; c += 4) {
-          m0 = fmaxf(m0, fmaxf(__uint_as_float(sr0[c]), __uint_as_float(sr1[c])));
-          m1 = fmaxf(m1, fmaxf(__uint_as_float(sr0[c + 1]), __uint_as_float(sr1[c + 1])));
-          m2 = fmaxf(m2, fmaxf(__uint_as_float(sr0[c + 2]), __uint_as_float(sr1[c + 2])));
-          m3 = fmaxf(m3, fmaxf(__uint_as_float(sr0[c + 3]), __uint_as_float(sr1[c + 3])));
+      for (int i = 0; i < 32; i += 2) {
+        const int h = (i >> 1) & 1;
+        const float p0 = ex2_ftz(fmaf(sc[i], sl2e, -base[h]));
+        const float p1 = ex2_ftz(fmaf(sc[i + 1], sl2e, -base[h]));
+        l_run[h] += p0 + p1;
+        split_hi_lo(p0, p1, ph[i >> 1], pl[i >> 1]);
+      }
+      mbar_wait_mma(&bars->v_full[s], par);
+      {
+        const uint32_t v_addr = smem_u32(v_smem + s * PF_KT_BYTES);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < PF_KEYS / 16; ++kk) {   // 16 keys per MMA
+          // V tile: [64 keys][64 dims] per dim half, dims contiguous (MN-major): LBO = the next 64 dims,
+          // SBO = the next 8 keys
+          const uint64_t b_desc = gmma_desc_sw128(v_addr + kk * 16 * 128, PF_HALF_BYTES, 1024);
+          const uint32_t fh[4] = {ph[4 * kk], ph[4 * kk + 1], ph[4 * kk + 2], ph[4 * kk + 3]};
+          const uint32_t fl[4] = {pl[4 * kk], pl[4 * kk + 1], pl[4 * kk + 2], pl[4 * kk + 3]};
+          wgmma_bf16_rs_n128_mn(o, fh, b_desc, 1u);
+          wgmma_bf16_rs_n128_mn(o, fl, b_desc, 1u);
         }
-        mx = fmaxf(fmaxf(m0, m1), fmaxf(m2, m3));
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_regs(o);
       }
-      const float cand = mx * sl2e;
-      // lazy rescale: keep the old base unless the max grew by more than 2^8 (or there was none)
-      float corr = 1.0f;
-      bool need = false;
-      if (m_run == -INFINITY) {
-        m_run = cand;                        // first visible key of this row (O and l are still 0)
-      } else if (cand > m_run + PF_RESCALE_LOG2) {
-        corr = ex2_ftz(m_run - cand);
-        m_run = cand;
-        need = true;
-      }
-      // O is only touched when some row of this warp rescales: only then wait for PV_{j-1}.  (Every
-      // phase <= j-2 of pv_done is complete once S_j is full — QK_j was issued after PV_{j-2} — so the
-      // parity of phase j-1 is unambiguous even though earlier phases were never waited for.)
-      if (j > 0 && __any_sync(0xffffffffu, need)) {
-        mbar_wait(&bars->pv_done, ((uint32_t)(j - 1)) & 1u);
-        tcgen05_fence_after();
-        {
-          l_run *= corr;
-#pragma unroll 1
-          for (int c0 = 0; c0 < HEAD_DIM; c0 += 32) {
-            uint32_t o[32];
-            tmem_ld_x32(tmem_base + lane_base + PF_COL_O + (uint32_t)c0, o);
-            tmem_ld_wait();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * corr);
-            tmem_st_x32(tmem_base + lane_base + PF_COL_O + (uint32_t)c0, o);
-          }
-          tmem_st_wait();
-        }
-      }
-      const float base = (m_run == -INFINITY) ? 0.f : m_run;
-      uint32_t ph[32], pl[32];   // columns 0..31 = P hi (keys 2c, 2c+1), columns 32..63 = P lo
-      float ls0 = 0.f, ls1 = 0.f;
-      const float nbase = -base;
-#pragma unroll
-      for (int c = 0; c < 32; c += 2) {
-        const float p0 = ex2_ftz(fmaf(__uint_as_float(sr0[c]), sl2e, nbase));
-        const float p1 = ex2_ftz(fmaf(__uint_as_float(sr0[c + 1]), sl2e, nbase));
-        ls0 += p0; ls1 += p1;
-        split_hi_lo(p0, p1, ph[c >> 1], pl[c >> 1]);
-      }
-#pragma unroll
-      for (int c = 0; c < 32; c += 2) {
-        const float p0 = ex2_ftz(fmaf(__uint_as_float(sr1[c]), sl2e, nbase));
-        const float p1 = ex2_ftz(fmaf(__uint_as_float(sr1[c + 1]), sl2e, nbase));
-        ls0 += p0; ls1 += p1;
-        split_hi_lo(p0, p1, ph[16 + (c >> 1)], pl[16 + (c >> 1)]);
-      }
-      l_run += ls0 + ls1;
-      tmem_st_x32(s_addr, ph);
-      tmem_st_x32(s_addr + 32, pl);
-      tmem_st_wait();
-      tcgen05_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->p_full[bsel]);
+      if (lane == 0) mbar_arrive(&bars->v_empty[s]);
     }
     // ---- epilogue: O / l -> bf16 -> global ----
-    // pv_done phases are only waited for on demand, so the parity wait must never be more than one
-    // phase behind: S_{n-1} full implies PV_{n-3} done, hence phase n-2 is the oldest that can still
-    // be pending — wait for it first, then for the last one.  (Waiting for phase n-1 alone would see
-    // the parity of a still-pending phase n-2 as "n-1 complete" and read O two MMAs early.)
-    if (n_tiles >= 2) mbar_wait(&bars->pv_done, ((uint32_t)(n_tiles - 2)) & 1u);
-    mbar_wait(&bars->pv_done, ((uint32_t)(n_tiles - 1)) & 1u);
-    tcgen05_fence_after();
-    const float inv = 1.0f / l_run;
-    __nv_bfloat16* orow = a.out + ((size_t)(a.q_start[b] + tq) * a.heads + (kh * G + g)) * HEAD_DIM;
-#pragma unroll 1
-    for (int c0 = 0; c0 < HEAD_DIM; c0 += 32) {
-      uint32_t o[32];
-      tmem_ld_x32(tmem_base + lane_base + PF_COL_O + (uint32_t)c0, o);
-      tmem_ld_wait();
-      if (valid) {
 #pragma unroll
-        for (int c = 0; c < 32; c += 8) {
-          uint4 v;
-          v.x = pack_bf16x2(__uint_as_float(o[c]) * inv, __uint_as_float(o[c + 1]) * inv);
-          v.y = pack_bf16x2(__uint_as_float(o[c + 2]) * inv, __uint_as_float(o[c + 3]) * inv);
-          v.z = pack_bf16x2(__uint_as_float(o[c + 4]) * inv, __uint_as_float(o[c + 5]) * inv);
-          v.w = pack_bf16x2(__uint_as_float(o[c + 6]) * inv, __uint_as_float(o[c + 7]) * inv);
-          *reinterpret_cast<uint4*>(orow + c0 + c) = v;
-        }
-      }
+    for (int h = 0; h < 2; ++h) {
+      float l = l_run[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      if (limit[h] == 0) continue;
+      const float inv = 1.0f / l;
+      __nv_bfloat16* orow = a.out + ((size_t)(a.q_start[b] + tq0 + tok[h]) * a.heads + (kh * G + head[h])) * HEAD_DIM;
+#pragma unroll
+      for (int c = 0; c < 16; ++c)
+        *reinterpret_cast<uint32_t*>(orow + 8 * c + 2 * (lane & 3)) =
+            pack_bf16x2(o[4 * c + 2 * h] * inv, o[4 * c + 2 * h + 1] * inv);
     }
-    tcgen05_fence_before();
-  }
-  __syncthreads();
-  if (warp == 1) {
-    tcgen05_fence_after();
-    tmem_dealloc(tmem_base, PF_TMEM_COLS);
   }
 }
 

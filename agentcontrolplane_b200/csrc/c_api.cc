@@ -42,7 +42,7 @@ static char* dup_string(const std::string& s, size_t* len) {
 
 extern "C" {
 
-const char* acp_infer_version(void) { return "acp_infer 0.1.0 sm_100a"; }
+const char* acp_infer_version(void) { return "acp_infer 0.1.0 sm_90a"; }
 
 int acp_infer_init(const char* config_json, acp_engine** out) {
   if (!out) return ACP_ERR_INVALID;

@@ -1,7 +1,6 @@
-// gemm.cu — host side of the tcgen05 GEMM: TMA descriptor construction and launch dispatch.
+// gemm.cu — host side of the wgmma GEMM: TMA descriptor construction and launch dispatch.
 #include "gemm.h"
-#include "gemm_tcgen05.cuh"
-#include "gemm_persistent.cuh"
+#include "gemm_wgmma.cuh"
 #include <cudaTypedefs.h>
 #include <mutex>
 #include <stdlib.h>
@@ -101,13 +100,6 @@ int gemm_pick_bn(int N) {
   return 256;
 }
 
-// ACP_GEMM_SHALLOW=0: wide tiles keep the deep ring / one CTA per SM (A/B switch)
-static bool shallow_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ACP_GEMM_SHALLOW"); v = (e && *e == '0') ? 0 : 1; }
-  return v == 1;
-}
-
 template <int BN, int EPI>
 static int launch_one(const GemmLaunch& g, const CUtensorMap& tx, cudaStream_t stream) {
   GemmArgs a;
@@ -116,14 +108,8 @@ static int launch_one(const GemmLaunch& g, const CUtensorMap& tx, cudaStream_t s
   a.group_ranges = g.groups > 0 ? g.group_ranges : nullptr;
   // grouped: g.N = the tile-list capacity in ROWS (moe_tile_cap * BN), grid.x walks the flat tile list
   dim3 grid((g.N + BN - 1) / BN, (g.M + GEMM_BM - 1) / GEMM_BM, g.groups > 0 ? 1 : g.splits);
-  cudaError_t e;
-  constexpr int kShallow = GemmCfg<BN>::kShallowStages;
-  if (kShallow != GemmCfg<BN>::kStages && shallow_enabled())
-    e = acp_launch(gemm_wx_kernel<BN, EPI, kShallow>, grid, dim3(GEMM_THREADS), GemmCfg<BN>::smem_bytes(kShallow),
-                   stream, *g.w, tx, a);
-  else
-    e = acp_launch(gemm_wx_kernel<BN, EPI>, grid, dim3(GEMM_THREADS), GemmCfg<BN>::kSmemBytes,
-                   stream, *g.w, tx, a);
+  cudaError_t e = acp_launch(gemm_wx_kernel<BN, EPI>, grid, dim3(GEMM_THREADS), GemmCfg<BN>::kSmemBytes,
+                             stream, *g.w, tx, a);
   if (e != cudaSuccess) {
     fprintf(stderr, "[acp_infer] gemm launch failed BN=%d EPI=%d: %s\n", BN, EPI,
             cudaGetErrorString(e));
@@ -149,71 +135,18 @@ static bool persistent_enabled() {
   return v == 1;
 }
 
-// ACP_GEMM_2CTA=0: prefill GEMMs stay on the 1-CTA persistent kernel (A/B switch; the cta_group::2 kernel is the
-// default since it measured +10..15 % at 8192 rows and +7 % on the bench line, profiles/r2_gemm_2cta.md)
-static bool two_cta_enabled() {
-  static int v = -1;
-  if (v < 0) { const char* e = getenv("ACP_GEMM_2CTA"); v = (e && *e == '0') ? 0 : 1; }
-  return v == 1;
-}
-
-template <int EPI>
-static int launch_persistent2(const GemmLaunch& g, cudaStream_t stream) {
-  GemmArgs a;
-  a.M = g.M; a.N = g.N; a.K = g.K; a.splits = 1; a.ld = g.ld; a.n_cap = g.n_cap;
-  a.out = g.out; a.amax_val = nullptr; a.amax_idx = nullptr; a.n_dev = g.n_dev;
-  a.group_ranges = nullptr;
-  const int m_pairs = (g.M + GEMM_BM - 1) / GEMM_BM / 2, n_tiles = (g.N + PGEMM_BN - 1) / PGEMM_BN;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(148);
-  cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = P2_SMEM;
-  cfg.stream = stream;
-  // co-resident CTA pairs (74 = one per TPC on a full B200); asked once per instantiation
-  static int max_clusters = 0;
-  if (max_clusters == 0) {
-    int n = 0;
-    if (cudaOccupancyMaxActiveClusters(&n, gemm_wx_persistent2_kernel<EPI>, &cfg) != cudaSuccess || n <= 0) n = 74;
-    max_clusters = n;
-  }
-  int clusters = m_pairs * n_tiles;
-  if (clusters > max_clusters) clusters = max_clusters;
-  cfg.gridDim = dim3(2 * clusters);
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = acp_pdl_enabled() ? 1 : 0;   // the cluster shape is compiled in (__cluster_dims__)
-  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wx_persistent2_kernel<EPI>, *g.w, g.x->x[3], a, m_pairs, n_tiles);
-  if (e != cudaSuccess) {
-    fprintf(stderr, "[acp_infer] 2-CTA persistent gemm launch failed EPI=%d: %s\n", EPI, cudaGetErrorString(e));
-    return -5;
-  }
-  return 0;
-}
-
 // Which kernel gemm_launch picks (pure host logic: tests/test_abi_cpu.py pins the defaults without a GPU):
-// prefill-sized problems (N > 256; bf16, fused-SwiGLU or ONE fp32 plane out; not grouped) run the persistent kernel with
-// double-buffered TMEM accumulators — the cta_group::2 flavour whenever the weight rows pair up (M % 256 == 0:
-// every matrix of the served models), the 1-CTA flavour otherwise.
-// Tensor-parallel shards: the 70B TP=8 and Mixtral EP=8 runs with the cta_group::2 kernel + the persistent fp32-plane
-// epilogue ended in a stuck rank after ~2e4 exchanges (profiles/r2_call13_8gpu.md) while 1e6 single-GPU launches
-// and the TP=4/8 tests are clean; until that is understood a shard keeps the kernels of the validated 8-GPU runs.
-static bool tp_env(const char* name) {
-  const char* e = getenv(name);
-  return e && *e == '1';
-}
+// prefill-sized problems (N > 256; bf16, fused-SwiGLU or ONE fp32 plane out; not grouped) run the persistent
+// kernel, everything else the tiled one.  bn_override < 0 forces the persistent kernel (test hook).
+// Tensor-parallel shards keep the fp32 plane of the row-parallel projections on the tiled kernel unless
+// ACP_TP_GEMM_PERSISTENT_F32=1.
 int gemm_path(const GemmLaunch& g) {
-  static const bool tp_2cta = tp_env("ACP_TP_GEMM_2CTA"), tp_f32 = tp_env("ACP_TP_GEMM_PERSISTENT_F32");
+  static const bool tp_f32 = [] { const char* e = getenv("ACP_TP_GEMM_PERSISTENT_F32"); return e && *e == '1'; }();
   const bool f32_ok = g.epi == EPI_F32 && g.splits == 1 && (!g.tp_shard || tp_f32);
-  if (g.N > 256 && g.bn_override == 0 && g.groups == 0 && persistent_enabled() &&
-      (g.epi == EPI_BF16 || g.epi == EPI_SWIGLU || f32_ok)) {
-    const bool want2 = g.two_cta >= 0 ? g.two_cta == 1 : (two_cta_enabled() && (!g.tp_shard || tp_2cta));
-    if (want2 && g.M % (2 * GEMM_BM) == 0) return GEMM_PATH_PERSISTENT_2CTA;
+  if (g.N > 256 && g.bn_override <= 0 && g.groups == 0 && (persistent_enabled() || g.bn_override < 0) &&
+      (g.epi == EPI_BF16 || g.epi == EPI_SWIGLU || f32_ok))
     return GEMM_PATH_PERSISTENT;
-  }
-  const int bn = g.bn_override ? g.bn_override : gemm_pick_bn(g.N);
-  return (bn >= 128 && shallow_enabled()) ? GEMM_PATH_TILED_SHALLOW : GEMM_PATH_TILED;
+  return GEMM_PATH_TILED;
 }
 
 template <int EPI>
@@ -224,8 +157,8 @@ static int launch_persistent(const GemmLaunch& g, cudaStream_t stream) {
   a.group_ranges = nullptr;
   const int m_tiles = (g.M + GEMM_BM - 1) / GEMM_BM, n_tiles = (g.N + PGEMM_BN - 1) / PGEMM_BN;
   int grid = m_tiles * n_tiles;
-  if (grid > 148) grid = 148;  // one persistent CTA per SM
-  cudaError_t e = acp_launch(gemm_wx_persistent_kernel<EPI>, dim3(grid), dim3(GEMM_THREADS), PGEMM_SMEM, stream,
+  if (grid > GEMM_SMS) grid = GEMM_SMS;  // one persistent CTA per SM
+  cudaError_t e = acp_launch(gemm_wx_persistent_kernel<EPI>, dim3(grid), dim3(GEMM_THREADS), PGemmCfg::kSmemBytes, stream,
                              *g.w, g.x->x[4], a, m_tiles, n_tiles);
   if (e != cudaSuccess) {
     fprintf(stderr, "[acp_infer] persistent gemm launch failed EPI=%d: %s\n", EPI, cudaGetErrorString(e));
@@ -242,12 +175,9 @@ int gemm_launch(const GemmLaunch& g, cudaStream_t stream) {
     case GEMM_PATH_PERSISTENT:
       return g.epi == EPI_BF16 ? launch_persistent<EPI_BF16>(g, stream)
              : g.epi == EPI_F32 ? launch_persistent<EPI_F32>(g, stream) : launch_persistent<EPI_SWIGLU>(g, stream);
-    case GEMM_PATH_PERSISTENT_2CTA:
-      return g.epi == EPI_BF16 ? launch_persistent2<EPI_BF16>(g, stream)
-             : g.epi == EPI_F32 ? launch_persistent2<EPI_F32>(g, stream) : launch_persistent2<EPI_SWIGLU>(g, stream);
     default: break;
   }
-  const int bn = g.bn_override ? g.bn_override : gemm_pick_bn(g.N);
+  const int bn = g.bn_override > 0 ? g.bn_override : gemm_pick_bn(g.N);
   switch (bn) {
     case 16: return launch_bn<16>(g, g.x->x[0], stream);
     case 32: return launch_bn<32>(g, g.x->x[1], stream);
@@ -260,14 +190,8 @@ int gemm_launch(const GemmLaunch& g, cudaStream_t stream) {
 
 template <int BN, int EPI>
 static int set_attr() {
-  cudaError_t e = cudaFuncSetAttribute(gemm_wx_kernel<BN, EPI>,
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       GemmCfg<BN>::kSmemBytes);
-  constexpr int kShallow = GemmCfg<BN>::kShallowStages;
-  if (e == cudaSuccess && kShallow != GemmCfg<BN>::kStages)
-    e = cudaFuncSetAttribute(gemm_wx_kernel<BN, EPI, kShallow>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             GemmCfg<BN>::smem_bytes(kShallow));
-  return e == cudaSuccess ? 0 : -5;
+  return cudaFuncSetAttribute(gemm_wx_kernel<BN, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                              GemmCfg<BN>::kSmemBytes) == cudaSuccess ? 0 : -5;
 }
 template <int BN>
 static int set_attr_bn() {
@@ -277,12 +201,9 @@ static int set_attr_bn() {
 int gemm_setup_attributes() {
   int rc = set_attr_bn<16>() | set_attr_bn<32>() | set_attr_bn<64>() | set_attr_bn<128>() |
            set_attr_bn<256>();
-  if (cudaFuncSetAttribute(gemm_wx_persistent2_kernel<EPI_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, P2_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGEMM_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(gemm_wx_persistent2_kernel<EPI_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, P2_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(gemm_wx_persistent2_kernel<EPI_SWIGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, P2_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGEMM_SMEM) != cudaSuccess ||
-      cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_SWIGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGEMM_SMEM) != cudaSuccess)
+  if (cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_F32>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGemmCfg::kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_BF16>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGemmCfg::kSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI_SWIGLU>, cudaFuncAttributeMaxDynamicSharedMemorySize, PGemmCfg::kSmemBytes) != cudaSuccess)
     rc = -5;
   if (rc != 0) fprintf(stderr, "[acp_infer] cudaFuncSetAttribute(max dyn smem) failed\n");
   return rc;

@@ -1,4 +1,4 @@
-// gemm.h — host interface of the tcgen05 GEMM (see gemm_tcgen05.cuh for the kernel).
+// gemm.h — host interface of the wgmma GEMM (see gemm_wgmma.cuh for the kernels).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -35,12 +35,10 @@ struct GemmLaunch {
   float* amax_val = nullptr;
   int* amax_idx = nullptr;
   const int* n_dev = nullptr;
-  int bn_override = 0;  // 0 = pick from N
-  // a tensor-parallel shard's GEMM: keeps the kernels the 8-GPU runs were validated with (1-CTA persistent kernel,
-  // tiled kernel for the fp32 plane of the row-parallel projections) unless ACP_TP_GEMM_2CTA=1 /
-  // ACP_TP_GEMM_PERSISTENT_F32=1 — see gemm.cu gemm_path
+  int bn_override = 0;  // 0 = pick from N; < 0 = force the persistent kernel (N > 256)
+  // a tensor-parallel shard's GEMM: the fp32 plane of the row-parallel projections stays on the tiled kernel
+  // unless ACP_TP_GEMM_PERSISTENT_F32=1 — see gemm.cu gemm_path
   bool tp_shard = false;
-  int two_cta = -1;     // prefill (N > 256) GEMMs: -1 = policy (gemm.cu two_cta_enabled), 0 = 1-CTA persistent kernel, 1 = cta_group::2 kernel
   // grouped mode (mixture of experts): `groups` weight tensors of M rows each, concatenated in `w`;
   // group g works on rows [ranges[2g], ranges[2g] + ranges[2g+1]) of x / out (device array, layout of
   // moe_dispatch_kernel incl. its flat tile list).  bn_override = the tile height the list was built for,
@@ -50,7 +48,7 @@ struct GemmLaunch {
 };
 int gemm_pick_bn(int N);
 int gemm_launch(const GemmLaunch& g, cudaStream_t stream);
-enum { GEMM_PATH_TILED = 0, GEMM_PATH_PERSISTENT = 1, GEMM_PATH_PERSISTENT_2CTA = 2, GEMM_PATH_TILED_SHALLOW = 3 };
+enum { GEMM_PATH_TILED = 0, GEMM_PATH_PERSISTENT = 1 };
 int gemm_path(const GemmLaunch& g);   // the kernel gemm_launch would pick for this problem
 int gemm_setup_attributes();  // cudaFuncSetAttribute for every instantiation (once per device)
 

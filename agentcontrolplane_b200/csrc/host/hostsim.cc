@@ -653,6 +653,8 @@ extern "C" int acp_hostsim_run(acp_engine* engine, const char* config_json, char
   long long window_sum = 0;
   int window_max = 0;
   const bool dry_run = cfg.get("dry_run").as_bool(false);   // sizes only: no Task is reconciled
+  // "outputs": true returns every root Task's final phase and Output (what the reconcile loop left in its status)
+  std::vector<std::pair<std::string, std::string>> outputs(cfg.get("outputs").as_bool(false) ? (size_t)std::max(0, n_tasks) : 0);
   for (int i = 0; i < n_tasks; ++i) {
     int this_user_len = user_len;
     if (mixed) {
@@ -874,6 +876,7 @@ extern "C" int acp_hostsim_run(acp_engine* engine, const char* config_json, char
         std::lock_guard<std::mutex> lk(lat_mu);
         task_ms.push_back(total_ms);
         ++phases[t.Status.Phase];
+        if (!outputs.empty()) outputs[(size_t)i] = {t.Status.Phase, t.Status.Output};
         if (t.Status.Phase == "Failed" && first_error.empty())
           first_error = name + ": " + (t.Status.Error.empty() ? t.Status.StatusDetail : t.Status.Error);
         uint64_t h = 1469598103934665603ull;
@@ -913,6 +916,16 @@ extern "C" int acp_hostsim_run(acp_engine* engine, const char* config_json, char
   for (auto& kv : phases) ph.set(kv.first, Json(kv.second));
   out.set("final_phases", ph);
   if (!first_error.empty()) out.set("first_error", Json(first_error));   // why the first Failed Task failed
+  if (!outputs.empty()) {
+    Json arr = Json::array();
+    for (auto& o : outputs) {
+      Json e = Json::object();
+      e.set("phase", Json(o.first));
+      e.set("output", Json(o.second));
+      arr.push(e);
+    }
+    out.set("outputs", arr);
+  }
   char dbuf[32];
   snprintf(dbuf, sizeof dbuf, "%016llx", (unsigned long long)digest);
   out.set("digest", Json(std::string(dbuf)));

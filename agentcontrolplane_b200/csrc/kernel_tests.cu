@@ -3,7 +3,7 @@
 #include "acp_infer_kernels.h"
 #include "common.cuh"
 #include "gemm.h"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include "attention.h"
 #include <string.h>
 #include <vector>
@@ -32,8 +32,7 @@ extern "C" int acp_kernel_device_count(void) {
 extern "C" int acp_kernel_gemm_path(int M, int N, int K, int splits, int epi, int bn) {
   GemmLaunch g;
   g.M = M; g.N = N; g.K = K; g.epi = epi; g.splits = splits;
-  g.bn_override = bn > 0 ? bn : 0;
-  g.two_cta = bn == -2 ? 1 : (bn == -1 ? 0 : -1);
+  g.bn_override = bn;
   return gemm_path(g);
 }
 
@@ -79,8 +78,7 @@ extern "C" int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int 
   g.w = &mw.w; g.x = &mx; g.M = M; g.N = N; g.K = Kp; g.splits = splits; g.epi = epi;
   g.ld = (epi == EPI_SWIGLU) ? M / 2 : M; g.n_cap = N;
   g.out = (epi == EPI_ARGMAX && out == nullptr) ? nullptr : dout.p;
-  g.amax_val = (float*)dval.p; g.amax_idx = (int*)didx.p; g.bn_override = bn > 0 ? bn : 0;
-  g.two_cta = bn == -2 ? 1 : (bn == -1 ? 0 : -1);   // hook-only: bn -2 / -1 force the 2-CTA / 1-CTA prefill kernel
+  g.amax_val = (float*)dval.p; g.amax_idx = (int*)didx.p; g.bn_override = bn;   // hook-only: bn -1 forces the persistent prefill kernel
   int rc = gemm_launch(g, 0);
   if (rc != 0) return rc;
   ACP_CUDA_CHECK(cudaDeviceSynchronize());
@@ -124,7 +122,7 @@ extern "C" int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int 
     cudaEventDestroy(e1);
   }
   if (iters > 0 && elapsed_ms != nullptr) {
-    const size_t flush_n = (size_t)64 << 20;  // 256 MiB of fp32 > 126 MB L2
+    const size_t flush_n = (size_t)64 << 20;  // 256 MiB of fp32 > 50 MB L2
     if (dflush.alloc(flush_n * 4)) return -5;
     ACP_CUDA_CHECK(cudaMemset(dflush.p, 0, flush_n * 4));
     cudaEvent_t e0, e1;

@@ -509,7 +509,7 @@ __global__ void gather_weight_kernel(__nv_bfloat16* __restrict__ out, size_t n,
 int launch_gather_weight(__nv_bfloat16* out, size_t n, const __nv_bfloat16* src, size_t src_elem0,
                          cudaStream_t s, const SynthMap& map) {
   if (n == 0) return 0;
-  gather_weight_kernel<<<148 * 8, 256, 0, s>>>(out, n, src, src_elem0, map);
+  gather_weight_kernel<<<132 * 8, 256, 0, s>>>(out, n, src, src_elem0, map);
   ACP_LAUNCH_CHECK("gather_weight");
   return 0;
 }
@@ -519,7 +519,7 @@ int launch_synth(__nv_bfloat16* out, size_t n, uint64_t seed, uint32_t tid, doub
   if (n == 0) return 0;
   const uint64_t base = seed + (uint64_t)tid * 0x9E3779B97F4A7C15ull;
   const float scale = (float)(std / 37837.22671196048);
-  synth_weight_kernel<<<148 * 8, 256, 0, s>>>(out, n, base, scale, plus_one, map);
+  synth_weight_kernel<<<132 * 8, 256, 0, s>>>(out, n, base, scale, plus_one, map);
   ACP_LAUNCH_CHECK("synth");
   return 0;
 }

@@ -1,7 +1,7 @@
 // kernels.cuh — host launchers of the HBM-bound (non-GEMM) kernels of the decode engine.
 // Every kernel that consumes a GEMM result accepts it either as bf16 [T][M] (prefill, split-K off)
 // or as `splits` fp32 partial planes [splits][n_cap][M] which it sums in index order before the
-// bf16 rounding — the deterministic split-K reduction (see gemm_tcgen05.cuh).
+// bf16 rounding — the deterministic split-K reduction (see gemm_wgmma.cuh).
 #pragma once
 #include "model_config.h"
 #include <cuda_runtime.h>

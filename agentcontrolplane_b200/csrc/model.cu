@@ -10,7 +10,7 @@
 #include "model.h"
 #include "safetensors.h"
 #include "common.cuh"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -127,9 +127,9 @@ static int dmalloc_t(std::vector<void*>& allocs, T** p, size_t count, bool zero 
 //   N <= 256 rows (one N tile): depends only on (M, K), never on the batch size, so a sequence's
 //   arithmetic does not change with what it happens to be batched with (prefill steps never split:
 //   see gemm()) — the batch-invariance the tests check.
-//   N > 256 rows (BASELINE config 2, B = 512): the GEMMs are tensor-bound and 5-7 fp32 planes of
+//   N > 256 rows (e.g. B = 512): the GEMMs are tensor-bound and 5-7 fp32 planes of
 //   512 rows cost more than the MMAs (r1: QKV 0.5, O 0.4 PFLOP/s); there the split only has to give
-//   every SM the same share: S minimises ceil(tiles * S / 148) / S.  Still a fixed function of
+//   every SM the same share: S minimises ceil(tiles * S / SMs) / S.  Still a fixed function of
 //   (M, K, number of N tiles) — deterministic run to run — but a sequence decoded inside a batch of
 //   more than 256 sums its K range in different pieces than inside a smaller batch
 //   ("strict_batch_invariance": true keeps the one-tile splits everywhere).
@@ -181,9 +181,8 @@ int Model::init(const ModelConfig& cfg, const ModelLimits& lim, int device, int 
   if (env) lim_.splitk_target_ctas = atoi(env);
   env = getenv("ACP_FUSE_SWIGLU");
   fuse_swiglu_ = env && *env == '1';
-  // Prefill: SwiGLU runs in the persistent gate/up GEMM's epilogue (paired-lane exchange, hidden
-  // behind the next tile's mainloop by the double-buffered TMEM accumulator): A/B on one box
-  // 471 -> 450 ms per 32768 prompt tokens.  ACP_FUSE_SWIGLU_PREFILL=0 restores the separate kernel.
+  // Prefill: SwiGLU runs in the persistent gate/up GEMM's epilogue (paired-lane exchange; the producer
+  // streams the next tile meanwhile).  ACP_FUSE_SWIGLU_PREFILL=0 restores the separate kernel.
   env = getenv("ACP_TP_SYNC_EVERY");
   tp_sync_every_ = (env && tp_size > 1) ? atoi(env) : 0;
   env = getenv("ACP_FUSE_SWIGLU_PREFILL");
@@ -662,7 +661,7 @@ int Model::forward(const StepInput& in) {
   for (int l = 0; l < c.layers; ++l) {
     Layer& L = layers_[l];
     GemmOut qkv, o, dn;
-    // investigation knob (profiles/r2_call13_8gpu.md, hypothesis 1): bound this shard's launch queue
+    // investigation knob (ACP_TP_SYNC_EVERY): bound this shard's launch queue
     if (tp_sync_every_ > 0 && l > 0 && l % tp_sync_every_ == 0) ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
     PROF("gemm_qkv", gemm(L.m_qkv, m_xn_, qkv_l_, c.hidden, T, in.decode, &qkv));
     if (!in.decode) {

@@ -133,7 +133,7 @@ class Model {
     __nv_bfloat16 *k_cache, *v_cache;
     TmaMaps m_qkv, m_o, m_gu, m_down;
     CUtensorMap tm_k, tm_v;       // box = one (page, kv head) block, both dim halves (decode kernels)
-    CUtensorMap tm_k32, tm_v32;   // box = one dim half of a page (tcgen05 prefill kernel)
+    CUtensorMap tm_k32, tm_v32;   // box = one dim half of a page (wgmma prefill kernel)
   };
   std::vector<Layer> layers_;
   __nv_bfloat16 *embed_ = nullptr, *lm_head_ = nullptr, *final_norm_ = nullptr;

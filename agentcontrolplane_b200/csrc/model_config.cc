@@ -104,21 +104,22 @@ int splitk_factor(int M, int K, int N, int target_ctas, bool strict) {
   int s;
   if (N > 256 && !strict) {
     // co-resident CTAs share an SM's tensor pipe, so the GEMM's time follows the busiest SM: minimise
-    // ceil(tiles * S / 148) / S (waves of one CTA per SM, each doing 1/S of K); ties -> fewer planes
+    // ceil(tiles * S / SMS) / S (waves of one CTA per SM, each doing 1/S of K); ties -> fewer planes
+    constexpr int SMS = 132;   // H100 SXM
     const int tiles = m_tiles * ((N + 255) / 256);
     s = 1;
     // (>= one tile per SM already: no split — the persistent kernel balances those itself, bf16 epilogue)
-    if (tiles < 148) {
+    if (tiles < SMS) {
       const int cap = max_s < 8 ? max_s : 8;
       double best = 1e30;
       for (int cand = 1; cand <= cap; ++cand) {
-        const double cost = (double)((tiles * cand + 147) / 148) / cand;
+        const double cost = (double)((tiles * cand + SMS - 1) / SMS) / cand;
         if (cost < best) best = cost;
       }
       // every extra plane is N x M fp32 written and re-read: take the FEWEST planes within 15 % of the best
-      // wave count (128 tiles: 1 plane at cost 1.0, not 8 planes at 0.875; 64 tiles: 2; 96 tiles: 3)
+      // wave count (128 tiles: 1 plane at cost 1.0, not 8 planes at 0.875; 64 tiles: 2; 96 tiles: 4)
       for (int cand = 1; cand <= cap; ++cand) {
-        const double cost = (double)((tiles * cand + 147) / 148) / cand;
+        const double cost = (double)((tiles * cand + SMS - 1) / SMS) / cand;
         if (cost <= best * 1.15 + 1e-9) { s = cand; break; }
       }
     }

@@ -1,6 +1,6 @@
 // moe.cu — sparse mixture-of-experts MLP (Mixtral): router, token dispatch, weighted combine.
 //
-// Per layer (T token rows, E experts, top-2; the expert GEMMs are the grouped mode of gemm_tcgen05.cuh):
+// Per layer (T token rows, E experts, top-2; the expert GEMMs are the grouped mode of gemm_wgmma.cuh):
 //   moe_router_kernel    r[t][e] = xn[t] . Wr[e] in a FIXED fp32 summation order (the oracle's
 //                        router_logits() restates it, so expert selection is bit-identical), top-2 by
 //                        logit (lowest index wins ties), w0 = 1/(1+exp(r1-r0)), w1 = exp(r1-r0)/(1+exp(r1-r0))
@@ -17,7 +17,7 @@
 // (Mixtral-8x7B); architecture = transformers MixtralSparseMoeBlock (oracle/llama_oracle.py _moe).
 #include "moe.h"
 #include "common.cuh"
-#include "gemm_tcgen05.cuh"
+#include "gemm_wgmma.cuh"
 
 namespace acp {
 
@@ -117,7 +117,7 @@ moe_dispatch_kernel(const int* __restrict__ topk_idx, int T, int e_first, int e_
       off += s_cnt[e][1024];
     }
     s_off[e_local] = off;
-    // flat work list of the grouped GEMMs (layout: GEMM_GROUP_TILES in gemm_tcgen05.cuh): one entry
+    // flat work list of the grouped GEMMs (layout: GEMM_GROUP_TILES in gemm_wgmma.cuh): one entry
     // {expert, first row inside the expert} per BN-row tile
     int n = 0;
     int* tiles = ranges + GEMM_GROUP_TILES + 2;

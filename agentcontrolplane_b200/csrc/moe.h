@@ -11,7 +11,7 @@ int launch_moe_router(const __nv_bfloat16* xn, const __nv_bfloat16* wr, int hidd
 // ranges[e_local][2] = {first row, rows} of each local expert in the expert-sorted buffers,
 // row_of[T][2] = row of each assignment (-1: the expert lives on another rank)
 // Also writes the flat tile list of the grouped GEMMs for N tiles of `bn` rows (layout: GEMM_GROUP_TILES in
-// gemm_tcgen05.cuh; at most moe_tile_cap(T, bn, e_local) entries).
+// gemm_wgmma.cuh; at most moe_tile_cap(T, bn, e_local) entries).
 int launch_moe_dispatch(const int* topk_idx, int T, int e_first, int e_local, int bn, int* ranges, int* row_of, cudaStream_t s);
 int moe_ranges_ints(int T);                       // size of the `ranges` array for steps of up to T rows
 int moe_tile_cap(int T, int bn, int e_local);     // upper bound of the tile count (grid.x of the grouped GEMMs)

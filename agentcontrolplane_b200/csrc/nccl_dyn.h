@@ -1,6 +1,6 @@
 // nccl_dyn.h — NCCL resolved with dlopen at run time (only engines with "tp" > 1 need it), so
 // libacp_infer.so has no link-time dependency on libnccl.  Single-process / one-comm-per-GPU use
-// (ncclCommInitAll); collectives run over NVLink 5 / NVSwitch.
+// (ncclCommInitAll); collectives run over NVLink / NVSwitch.
 #pragma once
 #include <cuda_runtime.h>
 #include <stddef.h>

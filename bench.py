@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench.py — the hot path of BASELINE.json: Task reconciles through `provider: local`.
 
-  python bench.py --gpus N --steps K --warmup W [--impl reference]
+  python bench.py --gpus N --steps K --warmup W [--impl reference] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch of synthetic Task CRs: BASELINE config 2 (the
 largest single-GPU configuration, the one nearest north_star's ">= 1000 concurrent Task CRs"):
-512 concurrent Tasks, context windows log-uniform on [128, 4096] tokens (seeded, mean ~1150),
+256 concurrent Tasks, context windows log-uniform on [128, 4096] tokens (seeded, mean ~1100; their KV
+cache, ~43 GB, and the 16 GB of weights fit one 80 GB H100),
 continuous batching, greedy, max_tokens 64, Llama-3-8B shapes with seeded synthetic bf16 weights (no
 checkpoints or network in this image).  Config 1 (64 Tasks x 512 tokens) is run on the same engine
 after the timed region and reported under the extra key "config1".  Every Task goes  Task CR JSON -> sendLLMRequest (C++ mirror of the reference's
@@ -22,6 +23,12 @@ Reported on ONE JSON line (rank 0):
   device time per decode step vs MEASURED_PEAKS.json hbm_gbs), roofline_prefill (algorithmic FLOPs of
   the prefill steps incl. causal attention / their device time vs bf16_tflops_sustained), cpu_baseline (the reference's CPU reconcile
   loop restated in C++ against a loopback stub completion server, same box, core count stated).
+
+--dump-outputs DIR: after the timed steps, writes what the last timed step returned to its caller — the
+final status of every root Task — as DIR/task_output_bytes.npy (float32 [tasks][longest Output]: the UTF-8
+bytes of each Task's Output, -1 past its end), DIR/task_output_len.npy (float32 [tasks]) and
+DIR/task_final_answer.npy (float32 [tasks]: 1 = phase FinalAnswer).  Inputs depend only on the arguments
+(seeded windows, seeded synthetic weights), so two builds can be compared output for output.
 
 N > 1: one engine replica per GPU (request-level data parallelism, no collective on the data
 path — DESIGN.md §6); weak scaling: every rank runs its own 64 Tasks; time = max over ranks.
@@ -47,10 +54,10 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 WORKLOADS = {
-    # BASELINE.json configs[2]: the largest single-GPU configuration (default since round 2)
-    2: {"name": "llama-3-8b provider:local, 512 concurrent Task CRs, context windows log-uniform 128..4096 tokens (mean ~1150), "
+    # BASELINE.json configs[2]: the largest single-GPU configuration (default)
+    2: {"name": "llama-3-8b provider:local, 256 concurrent Task CRs, context windows log-uniform 128..4096 tokens (mean ~1100), "
                 "continuous batching, greedy, max_tokens 64",
-        "model": "llama-3-8b", "tasks": 512, "prompt_tokens": 0, "prompt_min": 128, "prompt_max": 4096, "max_tokens": 64,
+        "model": "llama-3-8b", "tasks": 256, "prompt_tokens": 0, "prompt_min": 128, "prompt_max": 4096, "max_tokens": 64,
         "tp": 1, "tools": 0, "tool_loop": False},
     # BASELINE.json configs[1]: 64 Tasks x 512 tokens (round 1's driver line; now the "config1" extra key)
     1: {"name": "llama-3-8b provider:local, 64 concurrent Task CRs, 512-token context, greedy, max_tokens 64",
@@ -68,12 +75,6 @@ WORKLOADS = {
         "arrival_rate": 1024.0, "delegation_depth": 2},
 }
 WORKLOAD = WORKLOADS[2]
-# DRAM bytes of ONE decode step from the committed `ncu --set full` captures (dram__bytes_read + write)
-NCU_TRAFFIC = {1: 20.00e9, 2: 107.4e9}
-NCU_TRAFFIC_SOURCE = {1: "profiles/r1_v3_ncu_full_decode_kernels.md: 32 x (QKV 51.2 + attention 146.0 + O 34.1 "
-                         "+ gate/up 238.4 + down 122.3 MB) + LM head 1054.4 MB, ctx 515",
-                      2: "profiles/r2_config2_decode_ncu.md: 32 x 3321.8 MB (attention 2668.3 + merge 59.9 + gate/up 256.0 + O/down 193.2 "
-                         "+ QKV 56.2 + add_rmsnorm 58.8 + swiglu 29.4) + LM head 1.06 GB, B = 512"}
 
 
 def measured_peaks():
@@ -83,18 +84,18 @@ def measured_peaks():
             return float(json.load(open(path))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:  # noqa: BLE001
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not a measured rate"
 
 
 def measured_tensor_peak():
-    """Sustained dense bf16 TFLOP/s (the prefill GEMMs run inside a long step, B200_PROFILING.md)."""
+    """Sustained dense bf16 TFLOP/s (the prefill GEMMs run inside a long step)."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         try:
             return float(json.load(open(path))["bf16_tflops_sustained"]), "measured (MEASURED_PEAKS.json bf16_tflops_sustained)"
         except Exception:  # noqa: BLE001
             pass
-    return 1400.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16, 700 W), not a measured rate"
 
 
 def window_cfg(w: dict) -> dict:
@@ -217,6 +218,20 @@ def cpu_baseline_sample() -> dict:
             "single_worker_value": one["reconciles_per_s"], "p50_step_ms": r["step_ms_p50"]}
 
 
+def dump_outputs(out_dir: str, outputs: list) -> None:
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    data = [o["output"].encode("utf-8") for o in outputs]
+    width = max([len(d) for d in data] + [1])
+    arr = np.full((len(data), width), -1.0, np.float32)
+    for i, d in enumerate(data):
+        arr[i, :len(d)] = np.frombuffer(d, np.uint8)
+    np.save(os.path.join(out_dir, "task_output_bytes.npy"), arr)
+    np.save(os.path.join(out_dir, "task_output_len.npy"), np.array([len(d) for d in data], np.float32))
+    np.save(os.path.join(out_dir, "task_final_answer.npy"),
+            np.array([o["phase"] == "FinalAnswer" for o in outputs], np.float32))
+
+
 def main():
     global WORKLOAD
     ap = argparse.ArgumentParser()
@@ -230,7 +245,11 @@ def main():
                     help="BASELINE.json config index (2 = default; 1 = 64 x 512; 3 = 70B TP=8, 4 = Mixtral EP=8: ONE process on an 8-GPU box, --gpus 1)")
     ap.add_argument("--max-tokens-per-step", type=int, default=4096, help="engine knob: token rows per prefill step (4096 measured 1.3 %% faster than 8192)")
     ap.add_argument("--tp", type=int, default=0, help="dev only: override the tensor-parallel degree of --config 3")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the root Tasks' final outputs of the last timed step to DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     WORKLOAD = dict(WORKLOADS[args.config])
     if args.config in (3, 4):
         if args.model == WORKLOADS[1]["model"]:
@@ -318,7 +337,10 @@ def main():
     t0 = time.perf_counter()
     reconciles, p50s, phases, task_p50, task_p99 = 0, [], {}, [], []
     for i in range(args.steps):
-        r = host.hostsim_run(dict(sim, seed=i + 1), eng)
+        last = i == args.steps - 1 and args.dump_outputs is not None
+        r = host.hostsim_run(dict(sim, seed=i + 1, **({"outputs": True} if last else {})), eng)
+        if last:
+            dumped = r["outputs"]
         reconciles += r["reconciles"]
         p50s.append(r["step_ms_p50"])
         task_p50.append(r.get("task_ms_p50"))
@@ -421,7 +443,7 @@ def main():
                                        "x2 per layer over NVLink, tp_comm.cu)"),
                        "prefix_hits": s1.get("prefix_hits", 0), "prefix_tokens_reused": s1.get("prefix_tokens_reused", 0),
                        "l2": (f"inputs larger than L2: every decode step streams {s1['decode_bytes_algorithmic'] / max(1, s1['decode_steps']) / 1e9:.1f} GB "
-                              "of weights + KV (all GPUs) through a 126 MB L2 per GPU"),
+                              "of weights + KV (all GPUs) through a 50 MB L2 per GPU"),
                        "llm_steps_per_task": total_reconciles / (world * n_tasks * args.steps),
                        "final_phases": phases},
             "decode_tokens_per_s": total_decode_tokens / dec_max if dec_max > 0 else 0.0,  # all ranks / max decode time
@@ -438,9 +460,7 @@ def main():
                     "decode_tokens_per_s": total_decode_tokens / wall_max},
             "gpu_launches": launches,
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         # DRAM bytes of one decode step from the committed ncu --set full capture (config 1 only)
-                         "traffic": NCU_TRAFFIC.get(args.config) if not args.layers else None,
-                         "traffic_source": NCU_TRAFFIC_SOURCE.get(args.config),
+                         "traffic": None,
                          "peak_source": peak_src,
                          "kernel": "one decode step (all launches of the step, CUDA events on the engine stream)",
                          "bytes_per_decode_step": s1["decode_bytes_algorithmic"] / max(1, s1["decode_steps"]),
@@ -449,7 +469,7 @@ def main():
             # the other phase of the same timed region: prefill is dense contraction (tensor bound)
             "roofline_prefill": {"bound": "tensor", "achieved": pre_tf, "peak": tf_peak, "unit": "TFLOP/s",
                                  "frac": pre_tf / tf_peak, "traffic": None, "peak_source": tf_src,
-                                 "kernel": "all prefill steps (QKV/O/gate-up/down GEMMs on tcgen05 + causal paged attention + LM head rows), "
+                                 "kernel": "all prefill steps (QKV/O/gate-up/down GEMMs on wgmma + causal paged attention + LM head rows), "
                                            "CUDA events on the engine stream; FLOPs = 2 per layer weight per token + 4*head_dim per (query head, visible key)",
                                  "flops_per_prefill_token": s1.get("prefill_flops_algorithmic", 0.0) / max(1, s1["prefill_tokens"]),
                                  "prefill_tokens_timed": s1["prefill_tokens"],
@@ -463,6 +483,8 @@ def main():
         if world == 1 and args.config not in (3, 4):
             line["cpu_baseline"] = cpu_baseline_sample()
         print(json.dumps(line), flush=True)
+    if args.dump_outputs is not None and rank == 0:
+        dump_outputs(args.dump_outputs, dumped)
     if eng is not None:
         eng.close()
     if dist is not None:

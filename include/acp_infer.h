@@ -1,4 +1,4 @@
-/* acp_infer.h — C ABI of libacp_infer.so, the B200-native `provider: local` for ACP.
+/* acp_infer.h — C ABI of libacp_infer.so, the H100-native `provider: local` for ACP.
  *
  * This is the drop-in boundary for ONE path of humanlayer/agentcontrolplane: the Task reconciler's
  * per-step LLM call.  Everything the reference sends over HTTPS at
@@ -102,7 +102,7 @@ void acp_infer_free(void* p);
  * handle.  Must not run concurrently with any other call on `e`. */
 void acp_infer_shutdown(acp_engine* e);
 
-/* Library build info: "acp_infer <version> sm_100a". */
+/* Library build info: "acp_infer <version> sm_90a". */
 const char* acp_infer_version(void);
 
 #ifdef __cplusplus

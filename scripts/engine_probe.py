@@ -47,7 +47,7 @@ for rep in range(int(os.environ.get('REPS', '3'))):
     print(json.dumps({"rep": rep, "wall_s": round(wall, 3), "gen_tokens": ntok,
                       "reconciles_per_s": round(n_req / wall, 2),
                       "tp": s.get("tp", 1), "decode_tok_per_s": round(dec_tps, 1), "decode_GBps_per_gpu": round(gbs, 1),
-                      "frac_of_6590": round(gbs / 6590, 3),
+                      "frac_of_3350": round(gbs / 3350, 3),   # H100 SXM data sheet
                       "decode_step_ms_p50": s.get("decode_step_ms_p50"),
                       "prefill_ms": round(s["prefill_ms"], 2), "prefill_tokens": s["prefill_tokens"],
                       "prefill_tok_per_s": round(s["prefill_tokens"] / (s["prefill_ms"] / 1e3), 1) if s["prefill_ms"] else 0,

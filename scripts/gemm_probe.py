@@ -1,5 +1,7 @@
-"""Times the tcgen05 GEMM at the Llama-3-8B decode shapes (N = 64 live sequences) for a sweep
-of split-K factors.  Run under gpurun; writes gpurun_out/gemm_probe.json.  Dev tool only."""
+"""Times the wgmma GEMM at the Llama-3-8B decode shapes (N = 64 live sequences) for a sweep
+of split-K factors; prints one JSON line per (GEMM, N, split).  Needs a GPU.  Dev tool only.
+
+  python scripts/gemm_probe.py [N ...]"""
 import ctypes
 import json
 import os
@@ -23,7 +25,6 @@ def main():
         "lm_head": (128256, 4096, [1]),
     }
     Ns = [int(a) for a in sys.argv[1:]] or [64]
-    res = []
     for name, (M, K, splits_list) in shapes.items():
         w = rng.integers(0x3000, 0x3C00, size=(M, K), dtype=np.uint16)  # small positive bf16
         for N in Ns:
@@ -42,9 +43,6 @@ def main():
                 gbs = (M * K * 2) / (ms.value * 1e-3) / 1e9 if ms.value > 0 else 0
                 r = dict(gemm=name, M=M, K=K, N=N, splits=s, rc=rc, ms=ms.value, weight_GBps=gbs)
                 print(json.dumps(r), flush=True)
-                res.append(r)
-    os.makedirs("gpurun_out", exist_ok=True)
-    json.dump(res, open("gpurun_out/gemm_probe.json", "w"), indent=1)
 
 
 if __name__ == "__main__":

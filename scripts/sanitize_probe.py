@@ -1,5 +1,5 @@
 """Small end-to-end workload for compute-sanitizer (memcheck / racecheck / synccheck): every kernel of the
-engine runs at least once on the tiny presets — chunked prefill (tcgen05 attention), decode (per-item and
+engine runs at least once on the tiny presets — chunked prefill (wgmma attention), decode (per-item and
 chunked + merge attention, split-K GEMMs and their consumers, fused arg-max), sampling, logits, prefix
 pages — plus one launch of each unit-test hook.
 usage: compute-sanitizer --tool memcheck python scripts/sanitize_probe.py"""
@@ -39,12 +39,12 @@ for heads, kvh, q_len, ctx in ((4, 1, 70, 200), (8, 1, 33, 33)):
         rc = lib.acp_kernel_attn_prefill(q.ctypes.data_as(u16p), k.ctypes.data_as(u16p), v.ctypes.data_as(u16p), heads, kvh, q_len, ctx,
                                          impl, out.ctypes.data_as(u16p), 0, ctypes.byref(ms))
         assert rc == 0, rc
-# persistent prefill GEMM, 1-CTA and cta_group::2 (two N tiles, ragged), both epilogues
+# persistent and tiled prefill GEMM (two N tiles, ragged), both epilogues
 f32p, i32p = ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_int)
 for epi in (0, 3):
     w, x = bits((256, 128)), bits((300, 128))
     outs = []
-    for mode in (-1, -2):
+    for mode in (-1, 256):
         out = np.zeros((300, 128 if epi == 3 else 256), np.uint16)
         rc = lib.acp_kernel_gemm(w.ctypes.data_as(u16p), x.ctypes.data_as(u16p), 256, 300, 128, 1, epi, mode,
                                  out.ctypes.data_as(ctypes.c_void_p), None, None, 0, ctypes.byref(ms))

@@ -36,7 +36,7 @@ def test_expected_boundary_entry_points_present():
 def test_version_and_no_device_behaviour():
     lib = _lib.load()
     lib.acp_infer_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.acp_infer_version()
+    assert b"sm_90a" in lib.acp_infer_version()
     if lib.acp_kernel_device_count() == 0:
         with pytest.raises(EngineError) as ei:
             Engine({"model": "tiny"})
@@ -45,21 +45,21 @@ def test_version_and_no_device_behaviour():
 
 def test_default_kernel_dispatch():
     """The kernel the GEMM dispatcher picks by default, with no environment switch set (host logic, no GPU):
-    prefill-sized problems must run the persistent kernel, in its cta_group::2 flavour when the weight rows pair
-    up — an inverted default here silently costs 7-13 % of the bench (it happened once)."""
+    prefill-sized problems (more than 256 rows; bf16, SwiGLU or one fp32 plane) must run the persistent kernel,
+    everything else the tiled one — an inverted default here silently slows every prefill step."""
     import subprocess, sys
     code = (
         "import os\n"
-        "for k in ('ACP_GEMM_PERSISTENT', 'ACP_GEMM_2CTA', 'ACP_GEMM_SHALLOW'): os.environ.pop(k, None)\n"
+        "os.environ.pop('ACP_GEMM_PERSISTENT', None)\n"
         "from agentcontrolplane_b200 import _lib\n"
         "p = _lib.load().acp_kernel_gemm_path\n"
         "print(p(28672, 4096, 4096, 1, 3, 0), p(4096, 8192, 14336, 1, 0, 0), p(4096, 64, 4096, 1, 0, 0), p(4096, 256, 4096, 1, 0, 0),\n"
-        "      p(4096, 512, 4096, 2, 1, 0), p(8192, 4096, 1024, 1, 1, 0), p(4096, 4096, 4096, 1, 0, -2), p(4224, 4096, 4096, 1, 0, -2),\n"
-        "      p(4096, 4096, 4096, 1, 0, -1), p(4096, 4096, 4096, 1, 0, 256))\n")
+        "      p(4096, 512, 4096, 2, 1, 0), p(8192, 4096, 1024, 1, 1, 0), p(4224, 4096, 4096, 1, 0, 0),\n"
+        "      p(4096, 4096, 4096, 1, 0, -1), p(4096, 4096, 4096, 1, 0, 256), p(4096, 4096, 4096, 1, 2, 0))\n")
     out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, cwd=ROOT)
     assert out.returncode == 0, out.stderr
-    #          gate/up  down  decode  N=256  2 fp32 planes  1 fp32 plane (TP prefill)  2-CTA  odd m-tiles  1-CTA  forced tile
-    assert out.stdout.split() == ["2", "2", "0", "3", "3", "2", "2", "1", "1", "3"], out.stdout
+    #          gate/up  down  decode  N=256  2 fp32 planes  1 fp32 plane (TP prefill)  odd m-tiles  forced persistent  forced tile  arg-max
+    assert out.stdout.split() == ["1", "1", "0", "0", "0", "1", "1", "1", "0", "0"], out.stdout
 
 
 def test_product_never_imports_the_oracle():

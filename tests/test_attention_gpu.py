@@ -1,4 +1,4 @@
-"""Prefill attention kernels (agentcontrolplane_b200/csrc/attention_prefill_tc.cu — tcgen05 — and round 1's
+"""Prefill attention kernels (agentcontrolplane_b200/csrc/attention_prefill_tc.cu — wgmma — and round 1's
 mma.sync kernel) vs a numpy fp32 causal softmax attention, through the C-ABI test hook
 acp_kernel_attn_prefill (include/acp_infer_kernels.h): paged K/V with a shuffled page table, GQA group
 sizes 1..16, ragged lengths, chunk offsets (the query block starts in the middle of the context)."""
@@ -78,7 +78,7 @@ def test_prefill_attention_matches_fp32_reference(impl, heads, kv_heads, q_len, 
 
 def test_lazy_rescale_with_growing_scores():
     """Scores that keep growing along the context force the running max (and the lazy O rescale of
-    the tcgen05 kernel) to move many times; large |q| makes the softmax peaky."""
+    the wgmma kernel) to move many times; large |q| makes the softmax peaky."""
     rng = np.random.default_rng(99)
     q, k, v = _case(rng, 4, 1, 96, 700, qscale=3.0)
     kf = bits_to_f32(k)

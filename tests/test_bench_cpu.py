@@ -23,7 +23,7 @@ def test_reference_arm_contract():
     cb = j["cpu_baseline"]
     assert cb["kind"] == "port" and cb["cores"] >= 1 and cb["value"] == j["value"] and "sample" in cb
     assert j["e2e"] == {"value": j["value"], "unit": j["unit"], "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}
-    assert "512 concurrent Task CRs" in j["config"]["workload"] and "window tokens per step" in j["config"]["workload"]
+    assert "256 concurrent Task CRs" in j["config"]["workload"] and "window tokens per step" in j["config"]["workload"]
 
 
 def test_reference_arm_never_maps_the_product_library():

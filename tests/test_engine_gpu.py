@@ -11,10 +11,8 @@ pytestmark = pytest.mark.gpu
 SEED = 0xACB200
 # |engine - oracle(bf16 mode)| on fp32 logits.  Both round to bf16 at the same points; what is
 # left is fp32 summation order (tensor-core vs numpy) which can flip single bf16 roundings.  The bound
-# is stated relative to the logit scale: 8 % of the standard deviation of the oracle's logit vector
-# (measured: 0.010-0.020 at the hidden-512 presets whose logit std is 0.45, i.e. 2-4 %; 0.058 at the
-# real 8B width, logit std 1.28, i.e. 4.5 % — profiles/r2_fulldepth_noise.md), never looser than
-# LOGIT_ATOL absolute.
+# is stated relative to the logit scale: 8 % of the standard deviation of the oracle's logit vector,
+# never looser than LOGIT_ATOL absolute.
 LOGIT_ATOL = 3e-2
 LOGIT_RTOL = 8e-2
 

@@ -10,8 +10,8 @@ against two independent checkers that run as fp32 torch on the same GPU (test si
       answers).  HF has no bf16 rounding points, so this comparison is statistical (relative RMS logit
       error, correlation, arg-max agreement where HF's own margin clears the noise).
 
-Two weight regimes, because rounding noise behaves very differently in them (measured on a B200 with
-scripts/fulldepth_probe.py, profiles/r2_fulldepth_noise.md):
+Two weight regimes, because rounding noise behaves very differently in them (scripts/fulldepth_probe.py
+measures both):
 
   * DAMPED, w_std = 0.005 — every layer's update is of the order of the residual stream, as in a
     trained network.  bf16 rounding noise stays at ~1 % of the logit scale through all 32 layers
@@ -42,8 +42,8 @@ MODEL = "llama-3-8b"
 SEED = 0xACB200
 N_NEW = 6
 SAMPLE = [0, 9, 22, 37, 50, 63]
-# regime -> (max |engine - bf16 oracle| in units of the logit std, relative RMS vs HF fp32); measured 0.054 / 0.012
-# and 0.28 / 0.072 (profiles/r2_fulldepth_noise.md), bounds leave 2x head-room for other prompts
+# regime -> (max |engine - bf16 oracle| in units of the logit std, relative RMS vs HF fp32); the bounds leave
+# about 2x head-room over what scripts/fulldepth_probe.py reports, for other prompts
 REGIMES = {"damped": (0.005, 0.11, 0.03), "bench": (0.02, 0.6, 0.15)}
 
 

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (agentcontrolplane_b200/csrc/gemm_tcgen05.cuh) vs a numpy fp32 matmul of the same
+"""wgmma GEMM (agentcontrolplane_b200/csrc/gemm_wgmma.cuh) vs a numpy fp32 matmul of the same
 bf16 inputs, through the C-ABI test hook acp_kernel_gemm (include/acp_infer_kernels.h)."""
 import ctypes
 
@@ -45,7 +45,7 @@ def _rand_bits(rng, shape, scale):
     (512, 128, 256, 0), (256, 256, 192, 0), (256, 300, 128, 0),   # two N tiles, ragged
     (200, 20, 96, 0),                                              # ragged M, N, K
     (768, 5, 512, 0), (1024, 64, 4096, 0), (256, 7, 64, 64),
-    (2560, 2600, 192, 0),   # prefill-sized: persistent kernel, 220 tiles > 148 CTAs (several tiles per CTA, both TMEM buffers)
+    (2560, 2600, 192, 0),   # prefill-sized: persistent kernel, 220 tiles > 132 CTAs (several tiles per CTA)
     (384, 1000, 4096, 0),   # persistent kernel, long K (ring wraps many times per tile)
 ])
 def test_gemm_bf16_out(M, N, K, bn):
@@ -132,37 +132,46 @@ def test_gemm_fused_swiglu_epilogue(M, N, K):
     assert np.mean(err <= np.maximum(np.abs(ref) * 2.0 ** -7, 1e-3)) > 0.995
 
 
-# ---- cta_group::2 persistent prefill kernel (gemm_persistent.cuh gemm_wx_persistent2_kernel) ----------------
-# Same fp32 accumulation order as the 1-CTA kernel (K in order, one accumulator per output element), so the two
-# must agree BIT FOR BIT; the 1-CTA kernel is the one test_gemm_bf16_out pins against numpy.
+# ---- persistent prefill kernel (gemm_wgmma.cuh gemm_wx_persistent_kernel) vs the tiled kernel ----------------
+# Same fp32 accumulation order (K in order, one accumulator per output element), so the two must agree BIT FOR
+# BIT; the tiled kernel is the one test_gemm_bf16_out pins against numpy.
 @pytest.mark.parametrize("M,N,K,epi", [
-    (256, 300, 128, 0),       # one CTA pair, two N tiles (ragged: the second has 44 valid rows)
-    (256, 1000, 4096, 0),     # long K: the 6-stage ring wraps 10 times per tile
-    (2560, 2600, 192, 0),     # 10 pairs x 11 N tiles = 110 tiles > 74 clusters: both TMEM buffers, tile loop
+    (256, 300, 128, 0),       # two N tiles (ragged: the second has 44 valid rows)
+    (256, 1000, 4096, 0),     # long K: the ring wraps many times per tile
+    (2560, 2600, 192, 0),     # 20 m-tiles x 11 N tiles = 220 tiles > 132 CTAs: tile loop
     (4096, 8192, 4096, 0),    # Llama-3-8B wo at an 8192-token chunk
     (2048, 3000, 320, 3),     # fused SwiGLU epilogue
     (3584, 4096, 512, 3),
 ])
-def test_gemm_two_cta_matches_one_cta(M, N, K, epi):
+def test_gemm_persistent_matches_tiled(M, N, K, epi):
     rng = np.random.default_rng(M + 3 * N + K + epi)
     w = _rand_bits(rng, (M, K), 0.05)
     x = _rand_bits(rng, (N, K), 1.0)
-    one, _, _, _ = _gemm(w, x, epi=epi, bn=-1)
-    two, _, _, _ = _gemm(w, x, epi=epi, bn=-2)
-    assert np.array_equal(one, two), int(np.count_nonzero(one != two))
+    tiled, _, _, _ = _gemm(w, x, epi=epi, bn=256)
+    pers, _, _, _ = _gemm(w, x, epi=epi, bn=-1)
+    assert np.array_equal(tiled, pers), int(np.count_nonzero(tiled != pers))
     if epi == 0 and M * N <= 2560 * 2600:
         ref = bits_to_f32(x) @ bits_to_f32(w).T
-        got = bits_to_f32(two)
+        got = bits_to_f32(pers)
         assert np.all(np.abs(got - ref) <= np.maximum(np.abs(ref) * 2.0 ** -7, 1e-3))
+    if epi == 3:
+        # the SwiGLU epilogue both kernels share, against numpy (bounds of test_gemm_fused_swiglu_epilogue)
+        from oracle.bf16 import bf16_round
+        gu = bf16_round(bits_to_f32(x) @ bits_to_f32(w).T)
+        g, u = gu[:, 0::2], gu[:, 1::2]
+        ref = bf16_round(bf16_round(g / (np.float32(1.0) + np.exp(-g))) * u)
+        err = np.abs(bits_to_f32(pers) - ref)
+        assert np.all(err <= np.maximum(np.abs(ref) * 2.0 ** -5, 4e-3)), float(np.max(err))
+        assert np.mean(err <= np.maximum(np.abs(ref) * 2.0 ** -7, 1e-3)) > 0.995
 
 
-def test_gemm_two_cta_repeatable():
+def test_gemm_persistent_repeatable():
     rng = np.random.default_rng(11)
     w = _rand_bits(rng, (1024, 1024), 0.05)
     x = _rand_bits(rng, (5000, 1024), 1.0)
-    a, _, _, _ = _gemm(w, x, epi=0, bn=-2)
+    a, _, _, _ = _gemm(w, x, epi=0, bn=-1)
     for _ in range(3):
-        b, _, _, _ = _gemm(w, x, epi=0, bn=-2)
+        b, _, _, _ = _gemm(w, x, epi=0, bn=-1)
         assert np.array_equal(a, b)
 
 

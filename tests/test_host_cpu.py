@@ -239,6 +239,11 @@ def test_config0_plumbing_over_stub_server():
         r = host.hostsim_run({"tasks": 200, "workers": 4, "provider": "openai", "model": "gpt-4o", "baseURL": srv.base_url})
         assert r["reconciles"] == 200 and r["final_phases"] == {"FinalAnswer": 200}
         assert r["store_writes"] >= 4 * 200 and r["reconciles_per_s"] > 0
+        # "outputs": every root Task's final status, in Task order (what bench.py --dump-outputs writes)
+        r = host.hostsim_run({"tasks": 5, "workers": 2, "provider": "openai", "model": "gpt-4o", "baseURL": srv.base_url,
+                              "outputs": True})
+        assert r["outputs"] == [{"phase": "FinalAnswer", "output": "test"}] * 5
+        assert "outputs" not in host.hostsim_run({"tasks": 1, "provider": "openai", "model": "gpt-4o", "baseURL": srv.base_url})
     tool_body = G["G8_wire_fixtures"]["tool_body"]["body"]
     with host.StubServer(tool_body) as srv:
         out = host.task_step({"op": "sendLLMRequest", "task": _task(), "tools": B.convert_mcp_tools([{"name": "fetch"}], "fetch"),
@@ -499,10 +504,10 @@ def test_splitk_rule_and_workspace():
         assert len(small) == 1, (name, small)                      # (1)
         assert {f(M, K, n, 222, 1) for n in (300, 512, 1024)} == small, name   # strict mode keeps them everywhere
     assert (f(6144, 4096, 64, 222, 0), f(4096, 4096, 64, 222, 0), f(28672, 4096, 64, 222, 0), f(4096, 14336, 64, 222, 0)) == (5, 7, 1, 7)
-    # (2) B = 512 at Llama-3-8B (config 2): 96 / 64 / 448 / 64 tiles
-    assert (f(6144, 4096, 512, 222, 0), f(4096, 4096, 512, 222, 0), f(28672, 4096, 512, 222, 0), f(4096, 14336, 512, 222, 0)) == (3, 2, 1, 2)
+    # (2) B = 512 at Llama-3-8B: 96 / 64 / 448 / 64 tiles over 132 SMs
+    assert (f(6144, 4096, 512, 222, 0), f(4096, 4096, 512, 222, 0), f(28672, 4096, 512, 222, 0), f(4096, 14336, 512, 222, 0)) == (4, 2, 1, 2)
     assert f(4096, 4096, 1024, 222, 0) == 1                        # 128 tiles: one plane, not eight
-    assert f(4096, 4096, 2048, 222, 0) == 1                        # >= 148 tiles: never split
+    assert f(4096, 4096, 2048, 222, 0) == 1                        # >= 132 tiles: never split
     # (3) every step height fits the workspace, for every shape and both modes
     for name, (M, K) in shapes.items():
         for strict in (0, 1):

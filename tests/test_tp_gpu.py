@@ -1,6 +1,6 @@
 """Tensor parallelism (DESIGN.md §6): a TP=2 engine (one process, two GPUs, NCCL all-reduce over
 NVLink) must emit the same greedy tokens as the TP=1 engine and the oracle on the same synthetic
-weights.  Needs >= 2 GPUs (run with `gpurun --gpus 2`); skipped on a 1-GPU box."""
+weights.  Needs >= 2 GPUs; skipped on a 1-GPU machine."""
 import numpy as np
 import pytest
 
@@ -61,8 +61,7 @@ def test_tp_matches_tp1_and_oracle(tp, comm):
         lg_1 = e.logits(t, 1, 128256)
         e.result(t)
     # first-position logits: TP shards sum partial products in a different order (one rounding after the exchange).
-    # Bound: the engine tests' relative policy (8 % of the logit std, DESIGN.md §5); measured on B200: 0.010 at
-    # tiny-g2 TP=2, 0.040 / 0.037 at llama-3-8b-l2 TP=4 / 8 (logit std 1.3 -> bound 0.10)
+    # Bound: the engine tests' relative policy (8 % of the logit std, DESIGN.md §5)
     tol = max(3e-2, 0.08 * float(np.std(lg_1[0])))
     assert np.max(np.abs(lg_tp[0] - lg_1[0])) < tol, (float(np.max(np.abs(lg_tp[0] - lg_1[0]))), tol)
     for p, a, b in zip(prompts, got_tp, got_1):
