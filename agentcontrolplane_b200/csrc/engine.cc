@@ -128,6 +128,10 @@ int Engine::init(const char* config_json) {
   }
   model_name_ = name;
   tp_ = (int)cfg.get("tp").as_int(1);
+  if (mc.fp8 && tp_ != 1) {
+    fprintf(stderr, "[acp_infer] tp=%d: FP8 models run on one GPU (tp must be 1)\n", tp_);
+    return -1;
+  }
   if (tp_ < 1 || device + tp_ > ndev) {
     fprintf(stderr, "[acp_infer] tp=%d needs devices %d..%d but %d are visible\n", tp_, device, device + tp_ - 1, ndev);
     return -1;
@@ -900,6 +904,7 @@ std::string Engine::stats_json() {
   j.set("d2h_bytes", Json(model_.d2h_bytes()));
   j.set("tp", Json(tp_));
   j.set("weight_bytes_per_step", Json(c.weight_bytes()));
+  j.set("weight_dtype", Json(c.fp8 ? "fp8_e4m3" : "bf16"));
   j.set("kv_bytes_per_token", Json(c.kv_bytes_per_token()));
   // SURVEY.md §8(d): bytes_step = W + sum_seq ctx*K + B*K, summed over the decode steps so far
   // (whole model; with tp > 1 each GPU streams 1/tp of it)

@@ -22,6 +22,10 @@ int tma_encode_3d_bf16(CUtensorMap* out, const void* base, uint64_t d0, uint64_t
                        uint32_t box0, uint32_t box1, uint32_t box2);
 int tma_make_weight(TmaMaps* m, const void* base, uint64_t rows, uint64_t cols);
 int tma_make_act(TmaMaps* m, const void* base, uint64_t rows, uint64_t cols);
+// the same maps over e4m3 codes (one byte per element): weight tiles of 128 rows x 128 codes, activation
+// rows of `cols` codes
+int tma_make_weight_e4m3(TmaMaps* m, const void* base, uint64_t rows, uint64_t cols);
+int tma_make_act_e4m3(TmaMaps* m, const void* base, uint64_t rows, uint64_t cols);
 
 struct GemmLaunch {
   const CUtensorMap* w = nullptr;  // weight map (box 128 rows)
@@ -45,8 +49,14 @@ struct GemmLaunch {
   // N = tile capacity * bn_override (grid.x = capacity).
   int groups = 0;
   const int* group_ranges = nullptr;
+  // FP8: w / x are e4m3 maps, w_scale [M] per weight row, x_scale per activation row (DESIGN.md §5).
+  // Epilogues bf16, fp32 planes and SwiGLU; not grouped; N tiles of at most 128 tokens.
+  bool fp8 = false;
+  const float* w_scale = nullptr;
+  const float* x_scale = nullptr;
 };
 int gemm_pick_bn(int N);
+int gemm_pick_bn_e4m3(int N);
 int gemm_launch(const GemmLaunch& g, cudaStream_t stream);
 enum { GEMM_PATH_TILED = 0, GEMM_PATH_PERSISTENT = 1 };
 int gemm_path(const GemmLaunch& g);   // the kernel gemm_launch would pick for this problem

@@ -23,6 +23,13 @@
 // producer streams the next tile's stages while the consumers run the previous tile's epilogue.
 // Both flavours accumulate K in the same order, so they agree bit for bit.
 //
+// FP8 flavour (template flag FP8, the `-fp8` presets): W and X hold e4m3 codes, a k-block is still one
+// 128-byte swizzle row (now 128 elements) and a tile still 128 rows x 128 B, so the ring is unchanged;
+// each k-block issues four m64nBNk32 e4m3 MMAs into a scratch accumulator that is added to the fp32
+// accumulator on the CUDA cores once per k-block (DESIGN.md §4: FP8 wgmma keeps fewer accumulator bits
+// than fp32).  The epilogue scales by s_w[m] and then s_x[n] before the bf16 / fp32 / SwiGLU store.
+// The scratch accumulator doubles the registers, so FP8 tiles are at most 128 tokens wide.
+//
 // Reference boundary: this replaces the remote model behind
 // acp/internal/llmclient/langchaingo_client.go:102 (GenerateContent); see DESIGN.md.
 #pragma once
@@ -66,6 +73,9 @@ struct GemmArgs {
   // — all written on the device by moe_dispatch_kernel, so row counts never visit the host and
   // no CTA is launched for rows that do not exist (beyond the <= E slack of the grid bound).  splits must be 1.
   const int* group_ranges;
+  // FP8: per-row weight scales [M] and per-token activation scales (indexed like the activation rows)
+  const float* w_scale;
+  const float* x_scale;
 };
 
 template <int BN>
@@ -80,11 +90,13 @@ struct GemmCfg {
 };
 constexpr int PGEMM_BN = 256;
 using PGemmCfg = GemmCfg<PGEMM_BN>;
+constexpr int GEMM_BK_E4M3 = 128;   // e4m3 elements per k-block (the same 128-byte swizzle row)
+constexpr int PGEMM_BN_E4M3 = 128;
 
 // ---------------------------------------------------------------------------------
 // producer: the k-blocks [kb_begin, kb_end) of one tile into the ring (one thread)
 // ---------------------------------------------------------------------------------
-template <int BN, int STAGES>
+template <int BN, int STAGES, int BK = GEMM_BK>
 __device__ __forceinline__ void gemm_produce(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph,
                                              const CUtensorMap* tmap_w, const CUtensorMap* tmap_x, int w_row0, int kb_begin,
                                              int nkb, int x_row, uint64_t w_hint) {
@@ -94,7 +106,7 @@ __device__ __forceinline__ void gemm_produce(uint8_t* smem, uint64_t* full_bar, 
     uint8_t* a_dst = smem + s * Cfg::kStageBytes;
     mbar_arrive_expect_tx(&full_bar[s], Cfg::kStageBytes);
     tma_load_2d(a_dst, tmap_w, &full_bar[s], 0, w_row0 + (kb_begin + kb) * GEMM_BM, w_hint);
-    tma_load_2d(a_dst + Cfg::kABytes, tmap_x, &full_bar[s], (kb_begin + kb) * GEMM_BK, x_row, kEvictLast);
+    tma_load_2d(a_dst + Cfg::kABytes, tmap_x, &full_bar[s], (kb_begin + kb) * BK, x_row, kEvictLast);
     if (++s == STAGES) { s = 0; ph ^= 1; }
   }
 }
@@ -129,6 +141,52 @@ __device__ __forceinline__ void gemm_consume(float (&d)[BN / 2], uint8_t* smem, 
   wgmma_wait<0>();
   wgmma_fence_regs(d);
   if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+}
+
+// FP8 consumer: per k-block, four k32 MMAs into the scratch accumulator t (the first overwrites it), then
+// d += t in fp32 once they are done.  The stage is released right after the wait, before the adds.
+template <int BN, int STAGES>
+__device__ __forceinline__ void gemm_consume_e4m3(float (&d)[BN / 2], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
+                                                  int& s, uint32_t& ph, int nkb, int wg, int lane) {
+  using Cfg = GemmCfg<BN>;
+  float t[BN / 2];
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait_mma(&full_bar[s], ph);
+    const uint32_t a_addr = smem_u32(smem + s * Cfg::kStageBytes) + (uint32_t)wg * (64 * 128);
+    const uint64_t a_desc = gmma_desc_k_sw128(a_addr);
+    const uint64_t b_desc = gmma_desc_k_sw128(smem_u32(smem + s * Cfg::kStageBytes + Cfg::kABytes));
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BK_E4M3 / 32; ++k)
+      // 32 e4m3 = 32 bytes along K per MMA: +2 in the (addr >> 4) field, as for bf16
+      wgmma_e4m3_ss<BN>(t, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), k > 0 ? 1u : 0u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(t);
+    if (lane == 0) mbar_arrive(&empty_bar[s]);
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) d[i] += t[i];
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+}
+
+// FP8 dequantisation in the accumulator layout: d = fp32(fp32(d * s_w[m]) * s_x[n]) (rows / tokens past the
+// end are never stored, their scales are not read)
+template <int BN>
+__device__ __forceinline__ void gemm_scale_e4m3(float (&d)[BN / 2], const GemmArgs& args, int m_base, int n0, int row_off,
+                                                int n_valid, int lane) {
+  const int mr = m_base + (lane >> 2);
+  const int nc = n0 + 2 * (lane & 3);
+  const float sw0 = mr < args.M ? args.w_scale[mr] : 0.f;
+  const float sw8 = mr + 8 < args.M ? args.w_scale[mr + 8] : 0.f;
+#pragma unroll
+  for (int i = 0; i < BN / 2; ++i) {
+    const int n = nc + 8 * (i >> 2) + (i & 1);
+    const float sx = n < n_valid ? args.x_scale[row_off + n] : 0.f;
+    d[i] = __fmul_rn(__fmul_rn(d[i], ((i >> 1) & 1) ? sw8 : sw0), sx);
+  }
 }
 
 // ---------------------------------------------------------------------------------
@@ -232,12 +290,13 @@ __device__ __forceinline__ void gemm_store_argmax(const float (&d)[BN / 2], cons
 }
 
 // Tiled kernel: one CTA per (n-tile, m-tile, k-split).
-template <int BN, int EPI>
+template <int BN, int EPI, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, GemmCfg<BN>::kMinBlocks)
 gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                GemmArgs args) {
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::kStages;
+  constexpr int BK = FP8 ? GEMM_BK_E4M3 : GEMM_BK;
   extern __shared__ uint8_t smem_raw[];
   // 1024-byte alignment is required by the 128B swizzle atom (8 rows x 128 B).
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
@@ -266,7 +325,7 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
     m_tile = group * m_tiles + (int)blockIdx.y;
     split = 0;
   }
-  const int nkb_total = (args.K + GEMM_BK - 1) / GEMM_BK;
+  const int nkb_total = (args.K + BK - 1) / BK;
   const int kb_begin = (int)(((long long)nkb_total * split) / args.splits);
   const int kb_end = (int)(((long long)nkb_total * (split + 1)) / args.splits);
   const int nkb = kb_end - kb_begin;
@@ -298,10 +357,10 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
       // activations are re-read by every m-tile: evict-last
       for (int kb = 0; kb < pre; ++kb)
         tma_load_2d(smem + kb * Cfg::kStageBytes + Cfg::kABytes, &tmap_x, &full_bar[kb],
-                    (kb_begin + kb) * GEMM_BK, row_off + n0, kEvictLast);
+                    (kb_begin + kb) * BK, row_off + n0, kEvictLast);
       int s = pre % STAGES;
       uint32_t ph = (pre == STAGES) ? 1u : 0u;
-      gemm_produce<BN, STAGES>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_x, w_row0, kb_begin + pre, nkb - pre,
+      gemm_produce<BN, STAGES, BK>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_x, w_row0, kb_begin + pre, nkb - pre,
                                row_off + n0, kEvictFirst);
     }
   } else {
@@ -312,8 +371,10 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
     float d[BN / 2];
     int s = 0;
     uint32_t ph = 0;
-    gemm_consume<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+    if constexpr (FP8) gemm_consume_e4m3<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+    else gemm_consume<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
     const int m_base = m0 + cw * 16;
+    if constexpr (FP8) gemm_scale_e4m3<BN>(d, args, m_base, n0, row_off, n_valid, lane);
     if constexpr (EPI == EPI_ARGMAX) {
       asm volatile("bar.sync 1, 256;" ::: "memory");   // every MMA has read the ring: reuse it
       gemm_store_argmax<BN>(d, args, m_base, n0, n_valid, m_tile, cw, lane, smem);
@@ -325,20 +386,22 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
 
 // Persistent kernel (prefill): grid = min(tiles, SMs); tile t = (m-tile t / n_tiles, n-tile t % n_tiles),
 // n-tile fastest (CTAs running together share a weight tile; X stays in L2).  bf16, SwiGLU or one fp32 plane.
-template <int EPI>
+template <int EPI, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
                           GemmArgs args, int m_tiles, int n_tiles) {
-  constexpr int BN = PGEMM_BN;
-  constexpr int STAGES = PGemmCfg::kStages;
+  constexpr int BN = FP8 ? PGEMM_BN_E4M3 : PGEMM_BN;
+  using Cfg = GemmCfg<BN>;
+  constexpr int STAGES = Cfg::kStages;
+  constexpr int BK = FP8 ? GEMM_BK_E4M3 : GEMM_BK;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
-  uint64_t* full_bar = (uint64_t*)(smem + STAGES * PGemmCfg::kStageBytes);
+  uint64_t* full_bar = (uint64_t*)(smem + STAGES * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
-  const int nkb = (args.K + GEMM_BK - 1) / GEMM_BK;
+  const int nkb = (args.K + BK - 1) / BK;
   const int num_tiles = m_tiles * n_tiles;
 
   pdl_launch_dependents();
@@ -356,7 +419,7 @@ gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __gr
     if (threadIdx.x == 0) {
       pdl_wait();  // activations come from the previous kernel
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x)
-        gemm_produce<BN, STAGES>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_x, (t / n_tiles) * nkb * GEMM_BM, 0, nkb,
+        gemm_produce<BN, STAGES, BK>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_x, (t / n_tiles) * nkb * GEMM_BM, 0, nkb,
                                  (t % n_tiles) * BN, kEvictNormal);
     }
   } else {
@@ -365,7 +428,12 @@ gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __gr
     const int n_valid = args.n_dev ? *args.n_dev : args.N;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       float d[BN / 2];
-      gemm_consume<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+      if constexpr (FP8) {
+        gemm_consume_e4m3<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+        gemm_scale_e4m3<BN>(d, args, (t / n_tiles) * GEMM_BM + cw * 16, (t % n_tiles) * BN, 0, n_valid, lane);
+      } else {
+        gemm_consume<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+      }
       gemm_store<BN, EPI>(d, args, (t / n_tiles) * GEMM_BM + cw * 16, (t % n_tiles) * BN, 0, n_valid, 0, lane);
     }
   }

@@ -531,6 +531,13 @@ extern "C" size_t acp_host_splitk_workspace_bytes(int M, int K, int max_batch, i
   return acp::splitk_workspace_bytes(M, K, max_batch, target_ctas, strict != 0);
 }
 
+extern "C" int acp_host_splitk_factor_fp8(int M, int K, int N, int target_ctas, int strict) {
+  return acp::splitk_factor_fp8(M, K, N, target_ctas, strict != 0);
+}
+extern "C" size_t acp_host_splitk_workspace_bytes_fp8(int M, int K, int max_batch, int target_ctas, int strict) {
+  return acp::splitk_workspace_bytes_fp8(M, K, max_batch, target_ctas, strict != 0);
+}
+
 extern "C" int acp_host_checkpoint_index(const char* path, char** out_json) {
   if (!path || !out_json) return ACP_ERR_INVALID;
   acp::Checkpoint ck;
@@ -553,6 +560,7 @@ extern "C" int acp_host_checkpoint_index(const char* path, char** out_json) {
   m.set("kv_heads", Json(mc.kv_heads)); m.set("ffn", Json(mc.ffn)); m.set("vocab", Json(mc.vocab));
   m.set("rope_theta", Json(mc.rope_theta)); m.set("eps", Json((double)mc.eps));
   m.set("tied_embeddings", Json(mc.tied_embeddings)); m.set("max_pos", Json(mc.max_pos));
+  m.set("weight_dtype", Json(mc.fp8 ? "fp8_e4m3" : "bf16"));
   float inv[64];
   acp::rope_inv_freq(mc, inv);
   Json fr = Json::array();

@@ -5,6 +5,7 @@
 #include "gemm.h"
 #include "gemm_wgmma.cuh"
 #include "attention.h"
+#include "fp8.h"
 #include <string.h>
 #include <vector>
 
@@ -240,5 +241,96 @@ extern "C" int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, con
     cudaEventDestroy(e0);
     cudaEventDestroy(e1);
   }
+  return 0;
+}
+
+// mean milliseconds of `iters` launches, L2 flushed before each (two untimed warm-up launches)
+template <class F>
+static int time_launches(F launch, int iters, float* elapsed_ms) {
+  DevBuf dflush;
+  const size_t flush_n = (size_t)64 << 20;  // 256 MiB of fp32 > 50 MB L2
+  if (dflush.alloc(flush_n * 4)) return -5;
+  ACP_CUDA_CHECK(cudaMemset(dflush.p, 0, flush_n * 4));
+  cudaEvent_t e0, e1;
+  ACP_CUDA_CHECK(cudaEventCreate(&e0));
+  ACP_CUDA_CHECK(cudaEventCreate(&e1));
+  float total = 0.f;
+  int rc = 0;
+  for (int it = 0; it < iters + 2 && rc == 0; ++it) {
+    l2_flush_kernel<<<1184, 256>>>((float*)dflush.p, flush_n);
+    ACP_CUDA_CHECK(cudaEventRecord(e0, 0));
+    rc = launch();
+    ACP_CUDA_CHECK(cudaEventRecord(e1, 0));
+    ACP_CUDA_CHECK(cudaEventSynchronize(e1));
+    float ms = 0.f;
+    ACP_CUDA_CHECK(cudaEventElapsedTime(&ms, e0, e1));
+    if (it >= 2) total += ms;
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  *elapsed_ms = total / iters;
+  return rc;
+}
+
+extern "C" int acp_kernel_gemm_fp8(const uint8_t* w, const float* w_scale, const uint8_t* x, const float* x_scale, int M,
+                                   int N, int K, int splits, int epi, int bn, void* out, int iters, float* elapsed_ms) {
+  if (acp_kernel_device_count() <= 0) {
+    fprintf(stderr, "[acp_infer] no CUDA device: kernels cannot run (no CPU fallback)\n");
+    return -5;
+  }
+  if (!w || !w_scale || !x || !x_scale || !out || M <= 0 || N <= 0 || K <= 0 || epi == EPI_ARGMAX) return -1;
+  if (gemm_setup_attributes() != 0) return -5;
+  DevBuf dw, dx, dsw, dsx, dout;
+  const int n_pad = ((N + 255) / 256) * 256;
+  // zero codes pad M and K to (128, 128) multiples; weights go into the engine's tiled e4m3 layout
+  const int Mp = ((M + GEMM_BM - 1) / GEMM_BM) * GEMM_BM, Kp = ((K + GEMM_BK_E4M3 - 1) / GEMM_BK_E4M3) * GEMM_BK_E4M3;
+  const int nkb_p = Kp / GEMM_BK_E4M3;
+  std::vector<uint8_t> wt((size_t)Mp * Kp, 0), xp((size_t)n_pad * Kp, 0);
+  for (int r = 0; r < M; ++r)
+    for (int c = 0; c < K; ++c)
+      wt[((size_t)(r / GEMM_BM) * nkb_p + c / GEMM_BK_E4M3) * (GEMM_BM * GEMM_BK_E4M3) + (size_t)(r % GEMM_BM) * GEMM_BK_E4M3 +
+         c % GEMM_BK_E4M3] = w[(size_t)r * K + c];
+  for (int r = 0; r < N; ++r) memcpy(&xp[(size_t)r * Kp], &x[(size_t)r * K], (size_t)K);
+  if (dw.alloc(wt.size()) || dx.alloc(xp.size()) || dsw.alloc((size_t)Mp * 4) || dsx.alloc((size_t)n_pad * 4)) return -5;
+  ACP_CUDA_CHECK(cudaMemcpy(dw.p, wt.data(), wt.size(), cudaMemcpyHostToDevice));
+  ACP_CUDA_CHECK(cudaMemcpy(dx.p, xp.data(), xp.size(), cudaMemcpyHostToDevice));
+  ACP_CUDA_CHECK(cudaMemcpy(dsw.p, w_scale, (size_t)M * 4, cudaMemcpyHostToDevice));
+  ACP_CUDA_CHECK(cudaMemcpy(dsx.p, x_scale, (size_t)N * 4, cudaMemcpyHostToDevice));
+  size_t out_bytes = 0;
+  if (epi == EPI_BF16) out_bytes = (size_t)N * M * 2;
+  else if (epi == EPI_F32) out_bytes = (size_t)splits * N * M * 4;
+  else if (epi == EPI_SWIGLU) out_bytes = (size_t)N * (M / 2) * 2;
+  else return -1;
+  if (dout.alloc(out_bytes)) return -5;
+  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes));
+  TmaMaps mw, mx;
+  if (tma_make_weight_e4m3(&mw, dw.p, Mp, Kp) != 0) return -5;
+  if (tma_make_act_e4m3(&mx, dx.p, n_pad, Kp) != 0) return -5;
+  GemmLaunch g;
+  g.w = &mw.w; g.x = &mx; g.M = M; g.N = N; g.K = Kp; g.splits = splits; g.epi = epi;
+  g.ld = (epi == EPI_SWIGLU) ? M / 2 : M; g.n_cap = N; g.out = dout.p; g.bn_override = bn;
+  g.fp8 = true; g.w_scale = (const float*)dsw.p; g.x_scale = (const float*)dsx.p;
+  int rc = gemm_launch(g, 0);
+  if (rc != 0) return rc;
+  ACP_CUDA_CHECK(cudaDeviceSynchronize());
+  ACP_CUDA_CHECK(cudaMemcpy(out, dout.p, out_bytes, cudaMemcpyDeviceToHost));
+  if (iters > 0 && elapsed_ms != nullptr) return time_launches([&] { return gemm_launch(g, 0); }, iters, elapsed_ms);
+  return 0;
+}
+
+extern "C" int acp_kernel_quantize_fp8(const uint16_t* x, int rows, int cols, uint8_t* codes, float* scales) {
+  if (acp_kernel_device_count() <= 0) {
+    fprintf(stderr, "[acp_infer] no CUDA device: kernels cannot run (no CPU fallback)\n");
+    return -5;
+  }
+  if (!x || !codes || !scales || rows <= 0 || cols <= 0 || cols % 8) return -1;
+  DevBuf dx, dc, ds;
+  if (dx.alloc((size_t)rows * cols * 2) || dc.alloc((size_t)rows * cols) || ds.alloc((size_t)rows * 4)) return -5;
+  ACP_CUDA_CHECK(cudaMemcpy(dx.p, x, (size_t)rows * cols * 2, cudaMemcpyHostToDevice));
+  int rc = launch_quantize_rows_e4m3((const __nv_bfloat16*)dx.p, rows, cols, (uint8_t*)dc.p, (float*)ds.p, 0);
+  if (rc != 0) return rc;
+  ACP_CUDA_CHECK(cudaDeviceSynchronize());
+  ACP_CUDA_CHECK(cudaMemcpy(codes, dc.p, (size_t)rows * cols, cudaMemcpyDeviceToHost));
+  ACP_CUDA_CHECK(cudaMemcpy(scales, ds.p, (size_t)rows * 4, cudaMemcpyDeviceToHost));
   return 0;
 }

@@ -464,12 +464,14 @@ int launch_sample(const float* logits, int V, int N, const SampleParams* params_
 // ---------------------------------------------------------------------------------
 // Local element i of a (possibly tiled / interleaved / sharded) tensor -> index in the logical
 // row-major tensor whose values oracle/synth.py defines.
+// (TC = 128: the e4m3 tiles of the FP8 presets, 128 rows x 128 codes)
+template <int TC = 64>
 __device__ __forceinline__ size_t synth_logical_index(size_t i, const SynthMap& mp) {
   if (mp.local_cols <= 1) return i;
-  // storage is tiled: [m_tile][kb][128 rows][64 cols]  ->  local (row, col) of element i
-  const size_t nkb = (size_t)mp.local_cols / 64;
-  const size_t tile = i / 8192, in_tile = i % 8192;
-  const size_t r = (tile / nkb) * 128 + in_tile / 64, c = (tile % nkb) * 64 + in_tile % 64;
+  // storage is tiled: [m_tile][kb][128 rows][TC cols]  ->  local (row, col) of element i
+  const size_t nkb = (size_t)mp.local_cols / TC;
+  const size_t tile = i / (128 * TC), in_tile = i % (128 * TC);
+  const size_t r = (tile / nkb) * 128 + in_tile / TC, c = (tile % nkb) * TC + in_tile % TC;
   size_t lr;
   if (mp.interleave_half > 0) {
     lr = (size_t)mp.seg_global[r & 1] + (r >> 1);
@@ -511,6 +513,25 @@ int launch_gather_weight(__nv_bfloat16* out, size_t n, const __nv_bfloat16* src,
   if (n == 0) return 0;
   gather_weight_kernel<<<132 * 8, 256, 0, s>>>(out, n, src, src_elem0, map);
   ACP_LAUNCH_CHECK("gather_weight");
+  return 0;
+}
+
+// FP8 checkpoints: e4m3 codes through the same map into 128 x 128 tiles, and each row's scale to its row
+__global__ void gather_weight_e4m3_kernel(uint8_t* __restrict__ out, size_t n, const uint8_t* __restrict__ src,
+                                          float* __restrict__ s_out, int rows, const float* __restrict__ s_src, SynthMap mp) {
+  size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (; i < n; i += stride) out[i] = src[synth_logical_index<128>(i, mp)];
+  // local row r is element (r / 128, kb 0, row r % 128, col 0) of the tiling: its logical row = index / logical_cols
+  const size_t nkb = (size_t)mp.local_cols / 128;
+  for (size_t r = blockIdx.x * (size_t)blockDim.x + threadIdx.x; r < (size_t)rows; r += stride)
+    s_out[r] = s_src[synth_logical_index<128>((r / 128) * nkb * 16384 + (r % 128) * 128, mp) / (size_t)mp.logical_cols];
+}
+int launch_gather_weight_e4m3(uint8_t* out, size_t n, const uint8_t* src, float* s_out, int rows, const float* s_src,
+                              cudaStream_t s, const SynthMap& map) {
+  if (n == 0) return 0;
+  gather_weight_e4m3_kernel<<<132 * 8, 256, 0, s>>>(out, n, src, s_out, rows, s_src, map);
+  ACP_LAUNCH_CHECK("gather_weight_e4m3");
   return 0;
 }
 

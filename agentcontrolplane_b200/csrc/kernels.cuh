@@ -85,6 +85,11 @@ int launch_synth(__nv_bfloat16* out, size_t n, uint64_t seed, uint32_t tid, doub
 int launch_gather_weight(__nv_bfloat16* out, size_t n, const __nv_bfloat16* src, size_t src_elem0,
                          cudaStream_t s, const SynthMap& map);
 
+// FP8 checkpoints: row-major e4m3 codes `src` ([logical rows][logical_cols], the whole logical tensor) into the
+// 128 x 128-code tiles of `map`, and the fp32 scale of each of the `rows` local rows from s_src[logical row]
+int launch_gather_weight_e4m3(uint8_t* out, size_t n, const uint8_t* src, float* s_out, int rows, const float* s_src,
+                              cudaStream_t s, const SynthMap& map);
+
 // out[i] = sum_s planes[s][i] (index order), fp32 -> fp32: local split-K reduction in front of a
 // tensor-parallel all-reduce
 int launch_reduce_planes(const float* planes, int splits, size_t plane_elems, float* out, cudaStream_t s);

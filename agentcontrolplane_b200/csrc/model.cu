@@ -11,6 +11,7 @@
 #include "safetensors.h"
 #include "common.cuh"
 #include "gemm_wgmma.cuh"
+#include "fp8.h"
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -133,7 +134,10 @@ static int dmalloc_t(std::vector<void*>& allocs, T** p, size_t count, bool zero 
 //   (M, K, number of N tiles) — deterministic run to run — but a sequence decoded inside a batch of
 //   more than 256 sums its K range in different pieces than inside a smaller batch
 //   ("strict_batch_invariance": true keeps the one-tile splits everywhere).
+// FP8 GEMMs count k-blocks of 128 e4m3 elements (splitk_factor_fp8).  Still a function of (M, K) alone for one
+// N tile, so batch invariance holds under FP8 too.
 int Model::choose_splits(int M, int K, int N) const {
+  if (cfg_.fp8) return splitk_factor_fp8(M, K, N, lim_.splitk_target_ctas, lim_.strict_batch_invariance);
   return splitk_factor(M, K, N, lim_.splitk_target_ctas, lim_.strict_batch_invariance);   // model_config.cc
 }
 
@@ -150,6 +154,10 @@ int Model::init(const ModelConfig& cfg, const ModelLimits& lim, int device, int 
   if (cfg.heads % tp_size || cfg.kv_heads % tp_size || cfg.ffn % (64 * tp_size)) {
     fprintf(stderr, "[acp_infer] tp=%d does not divide heads=%d / kv_heads=%d / ffn=%d\n", tp_size,
             cfg.heads, cfg.kv_heads, cfg.ffn);
+    return -1;
+  }
+  if (cfg.fp8 && (tp_size > 1 || cfg.experts > 0 || cfg.hidden % 128 || cfg.ffn % 128)) {
+    fprintf(stderr, "[acp_infer] fp8 projections need a dense model on one GPU with hidden and ffn multiples of 128\n");
     return -1;
   }
   heads_l_ = cfg.heads / tp_size; kvh_l_ = cfg.kv_heads / tp_size;
@@ -209,8 +217,24 @@ int Model::alloc_all() {
   const size_t kv_elems = (size_t)lim_.num_pages * kvh_l_ * KV_PAGE * HEAD_DIM;
   for (int l = 0; l < c.layers; ++l) {
     Layer& L = layers_[l];
-    ACP_TRY(dmalloc_t(allocs_, &L.wqkv, (size_t)qkv_l_ * H));
-    ACP_TRY(dmalloc_t(allocs_, &L.wo, H * qdim_l_));
+    if (c.fp8) {
+      ACP_TRY(dmalloc_t(allocs_, &L.wqkv8, (size_t)qkv_l_ * H));
+      ACP_TRY(dmalloc_t(allocs_, &L.wo8, H * qdim_l_));
+      ACP_TRY(dmalloc_t(allocs_, &L.wgu8, (size_t)2 * ffn_l_ * H));
+      ACP_TRY(dmalloc_t(allocs_, &L.wdown8, H * ffn_l_));
+      ACP_TRY(dmalloc_t(allocs_, &L.s_qkv, (size_t)qkv_l_));
+      ACP_TRY(dmalloc_t(allocs_, &L.s_o, H));
+      ACP_TRY(dmalloc_t(allocs_, &L.s_gu, (size_t)2 * ffn_l_));
+      ACP_TRY(dmalloc_t(allocs_, &L.s_down, H));
+      ACP_TRY(tma_make_weight_e4m3(&L.m_qkv, L.wqkv8, qkv_l_, H));
+      ACP_TRY(tma_make_weight_e4m3(&L.m_o, L.wo8, H, qdim_l_));
+      ACP_TRY(tma_make_weight_e4m3(&L.m_gu, L.wgu8, 2 * ffn_l_, H));
+      ACP_TRY(tma_make_weight_e4m3(&L.m_down, L.wdown8, H, ffn_l_));
+      L.wqkv = L.wo = L.wgu = L.wdown = nullptr;
+    } else {
+      ACP_TRY(dmalloc_t(allocs_, &L.wqkv, (size_t)qkv_l_ * H));
+      ACP_TRY(dmalloc_t(allocs_, &L.wo, H * qdim_l_));
+    }
     if (c.experts > 0) {
       ACP_TRY(dmalloc_t(allocs_, &L.router, (size_t)c.experts * H));
       ACP_TRY(dmalloc_t(allocs_, &L.wgu_e, (size_t)experts_l_ * 2 * c.ffn * H));
@@ -218,7 +242,7 @@ int Model::alloc_all() {
       ACP_TRY(tma_make_weight(&L.m_gu_e, L.wgu_e, (uint64_t)experts_l_ * 2 * c.ffn, H));
       ACP_TRY(tma_make_weight(&L.m_down_e, L.wdown_e, (uint64_t)experts_l_ * H, c.ffn));
       L.wgu = L.wdown = nullptr;
-    } else {
+    } else if (!c.fp8) {
       ACP_TRY(dmalloc_t(allocs_, &L.wgu, (size_t)2 * ffn_l_ * H));
       ACP_TRY(dmalloc_t(allocs_, &L.wdown, H * ffn_l_));
     }
@@ -226,9 +250,11 @@ int Model::alloc_all() {
     ACP_TRY(dmalloc_t(allocs_, &L.ffn_norm, H));
     ACP_TRY(dmalloc_t(allocs_, &L.k_cache, kv_elems, true));
     ACP_TRY(dmalloc_t(allocs_, &L.v_cache, kv_elems, true));
-    ACP_TRY(tma_make_weight(&L.m_qkv, L.wqkv, qkv_l_, H));
-    ACP_TRY(tma_make_weight(&L.m_o, L.wo, H, qdim_l_));
-    if (c.experts == 0) {
+    if (!c.fp8) {
+      ACP_TRY(tma_make_weight(&L.m_qkv, L.wqkv, qkv_l_, H));
+      ACP_TRY(tma_make_weight(&L.m_o, L.wo, H, qdim_l_));
+    }
+    if (c.experts == 0 && !c.fp8) {
       ACP_TRY(tma_make_weight(&L.m_gu, L.wgu, 2 * ffn_l_, H));
       ACP_TRY(tma_make_weight(&L.m_down, L.wdown, H, ffn_l_));
     }
@@ -271,13 +297,25 @@ int Model::alloc_all() {
   ACP_TRY(tma_make_act(&m_attn_, attn_, T, qdim_l_));
   if (c.experts == 0) ACP_TRY(tma_make_act(&m_h_, h_, T, ffn_l_));
   ACP_TRY(tma_make_act(&m_xs_, xs_, Bp, H));
+  if (c.fp8) {
+    ACP_TRY(dmalloc_t(allocs_, &xn8_, (size_t)T * H, true));
+    ACP_TRY(dmalloc_t(allocs_, &attn8_, (size_t)T * qdim_l_, true));
+    ACP_TRY(dmalloc_t(allocs_, &h8_, (size_t)T * ffn_l_, true));
+    ACP_TRY(dmalloc_t(allocs_, &sx_xn_, (size_t)T, true));
+    ACP_TRY(dmalloc_t(allocs_, &sx_attn_, (size_t)T, true));
+    ACP_TRY(dmalloc_t(allocs_, &sx_h_, (size_t)T, true));
+    ACP_TRY(tma_make_act_e4m3(&m_xn8_, xn8_, T, H));
+    ACP_TRY(tma_make_act_e4m3(&m_attn8_, attn8_, T, qdim_l_));
+    ACP_TRY(tma_make_act_e4m3(&m_h8_, h8_, T, ffn_l_));
+  }
   // split-K workspace: worst case over the four GEMMs of a decode step with max_batch rows
   size_t ws = 0;
   const int shapes[4][2] = {{qkv_l_, c.hidden}, {c.hidden, qdim_l_}, {2 * ffn_l_, c.hidden}, {c.hidden, ffn_l_}};
   for (auto& s : shapes) {
     if (c.experts > 0 && (&s - shapes) >= 2) continue;   // the expert GEMMs are grouped, never split-K
     // the split factor depends on the row count beyond 256 rows: sized over every step height (model_config.cc)
-    const size_t b = splitk_workspace_bytes(s[0], s[1], lim_.max_batch, lim_.splitk_target_ctas, lim_.strict_batch_invariance);
+    const size_t b = c.fp8 ? splitk_workspace_bytes_fp8(s[0], s[1], lim_.max_batch, lim_.splitk_target_ctas, lim_.strict_batch_invariance)
+                           : splitk_workspace_bytes(s[0], s[1], lim_.max_batch, lim_.splitk_target_ctas, lim_.strict_batch_invariance);
     if (b > ws) ws = b;
   }
   if (tp_size_ > 1) {  // row-parallel GEMMs write fp32 (one rounding after the all-reduce), prefill too
@@ -318,7 +356,6 @@ int Model::gen_weights() {
   const ModelConfig& c = cfg_;
   const size_t H = c.hidden;
   // tensor ids shared with oracle/synth.py; SynthMap places this shard inside the logical tensors
-  const int r = tp_rank_;
   auto tiled = [&](int local_cols, int logical_cols, int col0) {
     SynthMap m;
     m.local_cols = local_cols; m.logical_cols = logical_cols; m.col0 = col0;
@@ -331,18 +368,54 @@ int Model::gen_weights() {
     ACP_TRY(launch_synth(lm_head_, (size_t)lm_rows_l_ * H, c.seed, 2, c.w_std, 0, stream_, m));
   }
   ACP_TRY(launch_synth(final_norm_, H, c.seed, 3, 0.1, 1, stream_));
-  for (int l = 0; l < c.layers; ++l) {
-    Layer& L = layers_[l];
+  // FP8 presets: each projection is generated in bf16 into one staging buffer, quantised row by row into its
+  // e4m3 tiles + scales, and the bf16 copy is freed at the end
+  __nv_bfloat16* stage = nullptr;
+  if (c.fp8) {
+    size_t n = (size_t)qkv_l_ * H;
+    if ((size_t)2 * ffn_l_ * H > n) n = (size_t)2 * ffn_l_ * H;
+    if (H * qdim_l_ > n) n = H * qdim_l_;
+    ACP_CUDA_CHECK(cudaMalloc((void**)&stage, n * sizeof(__nv_bfloat16)));
+  }
+  int rc = 0;
+  for (int l = 0; l < c.layers && rc == 0; ++l)
+    rc = gen_layer_weights(l, stage);
+  if (stage) {
+    ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    cudaFree(stage);
+  }
+  return rc;
+}
+
+// Layer l's synthetic tensors.  `stage` (FP8 presets) receives each bf16 projection before it is quantised.
+int Model::gen_layer_weights(int l, __nv_bfloat16* stage) {
+  const ModelConfig& c = cfg_;
+  const size_t H = c.hidden;
+  const int r = tp_rank_;
+  auto tiled = [&](int local_cols, int logical_cols, int col0) {
+    SynthMap m;
+    m.local_cols = local_cols; m.logical_cols = logical_cols; m.col0 = col0;
+    return m;
+  };
+  Layer& L = layers_[l];
+  {
     const uint32_t base = 16 + (uint32_t)l * 16;
+    auto dst = [&](__nv_bfloat16* w) { return stage ? stage : w; };
+    // FP8: quantise the projection just generated in `stage` (a tiled bf16 [M][K] matrix)
+    auto quant = [&](uint8_t* codes, float* scales, int M, int K) {
+      return stage ? launch_quantize_weight_e4m3(stage, M, K, codes, scales, stream_) : 0;
+    };
     {  // [q heads of this rank | k heads | v heads] rows of the logical [q | k | v] tensor
       SynthMap m = tiled((int)H, (int)H, 0);
       m.nseg = 3;
       m.seg_rows[0] = qdim_l_; m.seg_global[0] = r * qdim_l_;
       m.seg_rows[1] = kvdim_l_; m.seg_global[1] = c.q_dim() + r * kvdim_l_;
       m.seg_rows[2] = kvdim_l_; m.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
-      ACP_TRY(launch_synth(L.wqkv, (size_t)qkv_l_ * H, c.seed, base + 0, c.w_std, 0, stream_, m));
+      ACP_TRY(launch_synth(dst(L.wqkv), (size_t)qkv_l_ * H, c.seed, base + 0, c.w_std, 0, stream_, m));
+      ACP_TRY(quant(L.wqkv8, L.s_qkv, qkv_l_, (int)H));
     }
-    ACP_TRY(launch_synth(L.wo, H * qdim_l_, c.seed, base + 1, c.w_std, 0, stream_, tiled(qdim_l_, c.q_dim(), r * qdim_l_)));
+    ACP_TRY(launch_synth(dst(L.wo), H * qdim_l_, c.seed, base + 1, c.w_std, 0, stream_, tiled(qdim_l_, c.q_dim(), r * qdim_l_)));
+    ACP_TRY(quant(L.wo8, L.s_o, (int)H, qdim_l_));
     if (c.experts > 0) {
       // tensor ids of oracle/synth.py: router = layer_tid(l, 6); expert e: expert_tid(l, e, 0 = [gate; up] | 1 = down)
       ACP_TRY(launch_synth(L.router, (size_t)c.experts * H, c.seed, base + 6, c.w_std, 0, stream_));
@@ -361,9 +434,11 @@ int Model::gen_weights() {
         m.interleave_half = ffn_l_;
         m.seg_global[0] = r * ffn_l_;
         m.seg_global[1] = c.ffn + r * ffn_l_;
-        ACP_TRY(launch_synth(L.wgu, (size_t)2 * ffn_l_ * H, c.seed, base + 2, c.w_std, 0, stream_, m));
+        ACP_TRY(launch_synth(dst(L.wgu), (size_t)2 * ffn_l_ * H, c.seed, base + 2, c.w_std, 0, stream_, m));
+        ACP_TRY(quant(L.wgu8, L.s_gu, 2 * ffn_l_, (int)H));
       }
-      ACP_TRY(launch_synth(L.wdown, H * ffn_l_, c.seed, base + 3, c.w_std, 0, stream_, tiled(ffn_l_, c.ffn, r * ffn_l_)));
+      ACP_TRY(launch_synth(dst(L.wdown), H * ffn_l_, c.seed, base + 3, c.w_std, 0, stream_, tiled(ffn_l_, c.ffn, r * ffn_l_)));
+      ACP_TRY(quant(L.wdown8, L.s_down, (int)H, ffn_l_));
     }
     ACP_TRY(launch_synth(L.attn_norm, H, c.seed, base + 4, 0.1, 1, stream_));
     ACP_TRY(launch_synth(L.ffn_norm, H, c.seed, base + 5, 0.1, 1, stream_));
@@ -437,6 +512,55 @@ int Model::load_weights(const Checkpoint& ck) {
     return m;
   };
   auto whole = [&](const std::string& name, int64_t rows, int64_t cols) { return Part{name, rows, cols, 0, rows}; };
+  // FP8 (compressed-tensors float-quantized) projection: the `<name>.weight` F8_E4M3 codes of every part, stacked
+  // row-major in `stage`, and their `<name>.weight_scale` (BF16 / F32; [rows, 1] or [rows] per channel, a scalar
+  // per tensor, broadcast to every row) as fp32; then codes and scales are placed through the bf16 index map.
+  // Codes are used exactly as stored.
+  float* s_stage = nullptr;
+  std::vector<float> s_host;
+  if (c.fp8) {
+    size_t n = (size_t)c.qkv_dim();
+    if ((size_t)2 * c.ffn > n) n = (size_t)2 * c.ffn;
+    if (H > n) n = H;
+    ACP_CUDA_CHECK(cudaMalloc((void**)&s_stage, n * sizeof(float)));
+  }
+  auto upload_fp8 = [&](const std::vector<std::pair<std::string, int64_t>>& parts, int64_t cols, uint8_t* dst,
+                        float* s_dst, int local_rows, const SynthMap& m) -> int {
+    uint8_t* codes = (uint8_t*)stage;
+    int64_t row0 = 0;
+    s_host.clear();
+    for (const auto& pr : parts) {
+      const std::string wn = pr.first + ".weight", sn = pr.first + ".weight_scale";
+      const StTensor* t = ck.find(wn);
+      const StTensor* ts = ck.find(sn);
+      if (!t || !ts) { fprintf(stderr, "[acp_infer] checkpoint is missing %s\n", (!t ? wn : sn).c_str()); return -1; }
+      if (t->dtype != "F8_E4M3" || t->shape.size() != 2 || t->shape[0] != pr.second || t->shape[1] != cols) {
+        fprintf(stderr, "[acp_infer] %s: expected F8_E4M3 [%lld, %lld]\n", wn.c_str(), (long long)pr.second, (long long)cols);
+        return -1;
+      }
+      const int64_t ns = ts->numel();
+      const bool per_row = ns == pr.second && (ts->shape.size() == 1 || (ts->shape.size() == 2 && ts->shape[1] == 1));
+      if ((!per_row && ns != 1) || (ts->dtype != "F32" && ts->dtype != "BF16")) {
+        fprintf(stderr, "[acp_infer] %s: expected a BF16/F32 scale per output row or per tensor\n", sn.c_str());
+        return -1;
+      }
+      for (int64_t r = 0; r < pr.second; ++r) {
+        const int64_t e = per_row ? r : 0;
+        float v;
+        if (ts->dtype == "F32") memcpy(&v, ts->data + 4 * e, 4);
+        else { uint16_t b; memcpy(&b, ts->data + 2 * e, 2); const uint32_t u = (uint32_t)b << 16; memcpy(&v, &u, 4); }
+        s_host.push_back(v);
+      }
+      ACP_CUDA_CHECK(cudaMemcpyAsync(codes + (size_t)row0 * cols, t->data, t->nbytes, cudaMemcpyHostToDevice, stream_));
+      row0 += pr.second;
+    }
+    ACP_CUDA_CHECK(cudaMemcpyAsync(s_stage, s_host.data(), s_host.size() * sizeof(float), cudaMemcpyHostToDevice, stream_));
+    const size_t n = (size_t)local_rows * (size_t)m.local_cols;
+    int rc2 = launch_gather_weight_e4m3(dst, n, codes, s_dst, local_rows, s_stage, stream_, m);
+    if (rc2 != 0) return rc2;
+    ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    return 0;
+  };
   do {
     if ((rc = upload(whole("model.embed_tokens.weight", c.vocab, H), embed_)) != 0) break;
     {  // LM head: this shard's rows only (contiguous in the logical tensor)
@@ -452,6 +576,25 @@ int Model::load_weights(const Checkpoint& ck) {
     for (int l = 0; l < c.layers && rc == 0; ++l) {
       Layer& L = layers_[l];
       const std::string pre = "model.layers." + std::to_string(l) + ".";
+      if (c.fp8) {
+        SynthMap m = tiled((int)H, (int)H, 0);
+        m.nseg = 3;
+        m.seg_rows[0] = qdim_l_; m.seg_global[0] = r * qdim_l_;
+        m.seg_rows[1] = kvdim_l_; m.seg_global[1] = c.q_dim() + r * kvdim_l_;
+        m.seg_rows[2] = kvdim_l_; m.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
+        if ((rc = upload_fp8({{pre + "self_attn.q_proj", c.q_dim()}, {pre + "self_attn.k_proj", c.kv_dim()}, {pre + "self_attn.v_proj", c.kv_dim()}},
+                             H, L.wqkv8, L.s_qkv, qkv_l_, m)) != 0) break;
+        if ((rc = upload_fp8({{pre + "self_attn.o_proj", H}}, c.q_dim(), L.wo8, L.s_o, (int)H, tiled(qdim_l_, c.q_dim(), r * qdim_l_))) != 0) break;
+        m = tiled((int)H, (int)H, 0);
+        m.interleave_half = ffn_l_;
+        m.seg_global[0] = r * ffn_l_;
+        m.seg_global[1] = c.ffn + r * ffn_l_;
+        if ((rc = upload_fp8({{pre + "mlp.gate_proj", c.ffn}, {pre + "mlp.up_proj", c.ffn}}, H, L.wgu8, L.s_gu, 2 * ffn_l_, m)) != 0) break;
+        if ((rc = upload_fp8({{pre + "mlp.down_proj", H}}, c.ffn, L.wdown8, L.s_down, (int)H, tiled(ffn_l_, c.ffn, r * ffn_l_))) != 0) break;
+        if ((rc = upload(whole(pre + "input_layernorm.weight", H, 1), L.attn_norm)) != 0) break;
+        if ((rc = upload(whole(pre + "post_attention_layernorm.weight", H, 1), L.ffn_norm)) != 0) break;
+        continue;
+      }
       {  // logical [q; k; v]
         if ((rc = upload(whole(pre + "self_attn.q_proj.weight", c.q_dim(), H), stage)) != 0) break;
         if ((rc = upload(whole(pre + "self_attn.k_proj.weight", c.kv_dim(), H), stage + (size_t)c.q_dim() * H)) != 0) break;
@@ -508,6 +651,7 @@ int Model::load_weights(const Checkpoint& ck) {
     }
   } while (false);
   cudaFree(stage);
+  if (s_stage) cudaFree(s_stage);
   return rc;
 }
 
@@ -529,10 +673,12 @@ StepInput& Model::stage_begin(int T, int B, int n_blocks) {
   return s;
 }
 
-int Model::gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out) {
+int Model::gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out,
+                const float* w_scale, const float* x_scale) {
   GemmLaunch g;
   g.tp_shard = tp_size_ > 1;
   g.w = &w.w; g.x = &x; g.M = M; g.N = N; g.K = K;
+  g.fp8 = cfg_.fp8; g.w_scale = w_scale; g.x_scale = x_scale;
   const int splits = choose_splits(M, K, N);
   if (decode && splits > 1) {  // a single split writes bf16 directly (same rounding, half the bytes)
     g.epi = EPI_F32; g.splits = splits; g.out = ws_; g.ld = M; g.n_cap = N;
@@ -544,6 +690,11 @@ int Model::gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool de
   }
   ++launches_;
   return gemm_launch(g, stream_);
+}
+
+int Model::quantize_act(const __nv_bfloat16* x, int T, int cols, uint8_t* codes, float* scales) {
+  ++launches_;
+  return launch_quantize_rows_e4m3(x, T, cols, codes, scales, stream_);
 }
 
 // Row-parallel GEMM of a tensor-parallel shard (O and down projections): fp32 partial sums, local
@@ -663,7 +814,12 @@ int Model::forward(const StepInput& in) {
     GemmOut qkv, o, dn;
     // investigation knob (ACP_TP_SYNC_EVERY): bound this shard's launch queue
     if (tp_sync_every_ > 0 && l > 0 && l % tp_sync_every_ == 0) ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    PROF("gemm_qkv", gemm(L.m_qkv, m_xn_, qkv_l_, c.hidden, T, in.decode, &qkv));
+    if (c.fp8) {
+      PROF("quant_xn", quantize_act(xn_, T, c.hidden, xn8_, sx_xn_));
+      PROF("gemm_qkv", gemm(L.m_qkv, m_xn8_, qkv_l_, c.hidden, T, in.decode, &qkv, L.s_qkv, sx_xn_));
+    } else {
+      PROF("gemm_qkv", gemm(L.m_qkv, m_xn_, qkv_l_, c.hidden, T, in.decode, &qkv));
+    }
     if (!in.decode) {
       RopeKvArgs ra;
       ra.qkv = qkv; ra.pos = d_pos; ra.seq_of_row = d_seq; ra.page_table = d_pt;
@@ -703,7 +859,10 @@ int Model::forward(const StepInput& in) {
       PROF("gemm_o+p2p_allreduce_norm", rowpar_fused(L.m_o, m_attn_, qdim_l_, T, in.decode, L.ffn_norm, false));
     } else {
       if (tp_size_ > 1) PROF("gemm_o_allreduce", gemm_rowpar(L.m_o, m_attn_, c.hidden, qdim_l_, T, in.decode, &o));
-      else PROF("gemm_o", gemm(L.m_o, m_attn_, c.hidden, qdim_l_, T, in.decode, &o));
+      else if (c.fp8) {
+        PROF("quant_attn", quantize_act(attn_, T, qdim_l_, attn8_, sx_attn_));
+        PROF("gemm_o", gemm(L.m_o, m_attn8_, c.hidden, qdim_l_, T, in.decode, &o, L.s_o, sx_attn_));
+      } else PROF("gemm_o", gemm(L.m_o, m_attn_, c.hidden, qdim_l_, T, in.decode, &o));
       PROF("add_rmsnorm_o", launch_add_rmsnorm(x_, o, L.ffn_norm, xn_, nullptr, T, c.hidden, c.eps, stream_));
       ++launches_;
     }
@@ -718,6 +877,7 @@ int Model::forward(const StepInput& in) {
       }
       continue;
     }
+    if (c.fp8) PROF("quant_xn", quantize_act(xn_, T, c.hidden, xn8_, sx_xn_));
     if (fuse_swiglu_ || (!in.decode && T > 256 && fuse_swiglu_prefill_)) {
       // SwiGLU in the GEMM epilogue.  Decode (non-persistent kernel, epilogue exposed at the end of
       // every CTA) measured no gain, so it stays a separate kernel there unless ACP_FUSE_SWIGLU=1.
@@ -725,11 +885,13 @@ int Model::forward(const StepInput& in) {
       g.tp_shard = tp_size_ > 1;
       g.w = &L.m_gu.w; g.x = &m_xn_; g.M = 2 * ffn_l_; g.N = T; g.K = c.hidden; g.splits = 1;
       g.epi = EPI_SWIGLU; g.out = h_; g.ld = ffn_l_; g.n_cap = T;
+      if (c.fp8) { g.fp8 = true; g.x = &m_xn8_; g.w_scale = L.s_gu; g.x_scale = sx_xn_; }
       PROF("gemm_gateup_swiglu", gemm_launch(g, stream_));
       ++launches_;
     } else {
       GemmOut gu;
-      PROF("gemm_gateup", gemm(L.m_gu, m_xn_, 2 * ffn_l_, c.hidden, T, in.decode, &gu));
+      if (c.fp8) PROF("gemm_gateup", gemm(L.m_gu, m_xn8_, 2 * ffn_l_, c.hidden, T, in.decode, &gu, L.s_gu, sx_xn_));
+      else PROF("gemm_gateup", gemm(L.m_gu, m_xn_, 2 * ffn_l_, c.hidden, T, in.decode, &gu));
       PROF("swiglu", launch_swiglu(gu, h_, T, ffn_l_, stream_));
       ++launches_;
     }
@@ -745,7 +907,10 @@ int Model::forward(const StepInput& in) {
       continue;
     }
     if (tp_size_ > 1) PROF("gemm_down_allreduce", gemm_rowpar(L.m_down, m_h_, c.hidden, ffn_l_, T, in.decode, &dn));
-    else PROF("gemm_down", gemm(L.m_down, m_h_, c.hidden, ffn_l_, T, in.decode, &dn));
+    else if (c.fp8) {
+      PROF("quant_h", quantize_act(h_, T, ffn_l_, h8_, sx_h_));
+      PROF("gemm_down", gemm(L.m_down, m_h8_, c.hidden, ffn_l_, T, in.decode, &dn, L.s_down, sx_h_));
+    } else PROF("gemm_down", gemm(L.m_down, m_h_, c.hidden, ffn_l_, T, in.decode, &dn));
     if (l + 1 < c.layers) {
       PROF("add_rmsnorm_down", launch_add_rmsnorm(x_, dn, layers_[l + 1].attn_norm, xn_, nullptr, T, c.hidden, c.eps, stream_));
     } else {

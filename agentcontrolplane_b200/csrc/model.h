@@ -91,9 +91,13 @@ class Model {
  private:
   int alloc_all();
   int gen_weights();
+  int gen_layer_weights(int l, __nv_bfloat16* stage);
   int load_weights(const Checkpoint& ck);   // HuggingFace Llama safetensors -> tiled/sharded HBM layout
   int build_rope_tables();
-  int gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out);
+  // w_scale / x_scale: the FP8 presets' scales (w and x are then e4m3 maps)
+  int gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out,
+           const float* w_scale = nullptr, const float* x_scale = nullptr);
+  int quantize_act(const __nv_bfloat16* x, int T, int cols, uint8_t* codes, float* scales);
   int choose_splits(int M, int K, int N) const;
   int gemm_rowpar(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out);
 
@@ -131,7 +135,11 @@ class Model {
     __nv_bfloat16 *router = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;
     TmaMaps m_gu_e, m_down_e;
     __nv_bfloat16 *k_cache, *v_cache;
-    TmaMaps m_qkv, m_o, m_gu, m_down;
+    TmaMaps m_qkv, m_o, m_gu, m_down;   // over the e4m3 copies below when cfg.fp8
+    // FP8 presets: tiled e4m3 codes of the four projections (same row order as the bf16 matrices, which
+    // are then never allocated) and their fp32 per-row scales
+    uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *wgu8 = nullptr, *wdown8 = nullptr;
+    float *s_qkv = nullptr, *s_o = nullptr, *s_gu = nullptr, *s_down = nullptr;
     CUtensorMap tm_k, tm_v;       // box = one (page, kv head) block, both dim halves (decode kernels)
     CUtensorMap tm_k32, tm_v32;   // box = one dim half of a page (wgmma prefill kernel)
   };
@@ -143,6 +151,10 @@ class Model {
   __nv_bfloat16 *x_ = nullptr, *xn_ = nullptr, *qbuf_ = nullptr, *attn_ = nullptr, *h_ = nullptr,
                 *xs_ = nullptr, *gemm_bf16_ = nullptr;
   TmaMaps m_xn_, m_attn_, m_h_, m_xs_;
+  // FP8 presets: e4m3 copies of xn / attn / h (row-major) and their per-token scales
+  uint8_t *xn8_ = nullptr, *attn8_ = nullptr, *h8_ = nullptr;
+  float *sx_xn_ = nullptr, *sx_attn_ = nullptr, *sx_h_ = nullptr;
+  TmaMaps m_xn8_, m_attn8_, m_h8_;
   CUtensorMap tm_q_;   // qbuf_ as {128 dims, heads, rows} for the prefill attention's Q tiles
   float* ws_ = nullptr;  // split-K partial planes
   size_t ws_bytes_ = 0;

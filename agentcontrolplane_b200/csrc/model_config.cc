@@ -5,6 +5,18 @@
 namespace acp {
 
 bool model_preset(const std::string& name, ModelConfig* c) {
+  // "<dense preset>-fp8": the same shapes and seeded weights, projections quantised to e4m3 at init
+  const std::string sfx = "-fp8";
+  if (name.size() > sfx.size() && name.compare(name.size() - sfx.size(), sfx.size(), sfx) == 0) {
+    ModelConfig m;
+    if (!model_preset(name.substr(0, name.size() - sfx.size()), &m) || m.fp8 || m.experts > 0 || m.name == "sim" ||
+        m.name == "llama-3-70b")
+      return false;
+    m.name = name;
+    m.fp8 = true;
+    *c = m;
+    return true;
+  }
   ModelConfig m;
   m.name = name;
   if (name == "tiny") { m.hidden = 512; m.layers = 2; m.heads = 4; m.kv_heads = 1; m.ffn = 1024; }
@@ -42,6 +54,48 @@ void rope_inv_freq(const ModelConfig& c, float* inv64) {
     }
     inv64[i] = (float)f;
   }
+}
+
+// The one quantization_config this engine serves: compressed-tensors FP8_DYNAMIC (e4m3 weights with a per-channel
+// or per-tensor scale, activations quantised per token at run time, lm_head left in bf16).  Anything else is refused
+// with the offending field named.
+static bool parse_fp8_quantization(const Json& q, std::string* err) {
+  auto bad = [&](const std::string& field, const std::string& why) {
+    *err = "config.json: quantization_config." + field + " " + why;
+    return false;
+  };
+  const std::string method = q.get("quant_method").as_string();
+  if (method != "compressed-tensors") return bad("quant_method", "\"" + method + "\" is not supported (compressed-tensors)");
+  if (q.get("format").as_string() != "float-quantized")
+    return bad("format", "\"" + q.get("format").as_string() + "\" is not supported (float-quantized)");
+  if (!q.get("kv_cache_scheme").is_null()) return bad("kv_cache_scheme", "is not supported (the KV cache stays bf16)");
+  const Json& groups = q.get("config_groups");
+  if (!groups.is_object() || groups.size() != 1) return bad("config_groups", "must hold exactly one group");
+  const std::string gname = groups.members()[0].first;
+  const Json& g = groups.members()[0].second;
+  const std::string pre = "config_groups." + gname + ".";
+  const Json& tg = g.get("targets");
+  if (!tg.is_array() || tg.size() != 1 || tg.items()[0].as_string() != "Linear") return bad(pre + "targets", "must be [\"Linear\"]");
+  if (!g.get("output_activations").is_null()) return bad(pre + "output_activations", "is not supported");
+  auto check = [&](const char* which, const char* strategy, bool dynamic) {
+    const Json& a = g.get(which);
+    const std::string p = pre + which;
+    if (!a.is_object()) return bad(p, "is missing");
+    if (a.get("type").as_string() != "float") return bad(p + ".type", "\"" + a.get("type").as_string() + "\" is not supported (float)");
+    if (a.get("num_bits").as_int(0) != 8) return bad(p + ".num_bits", "must be 8");
+    const std::string st = a.get("strategy").as_string();
+    const bool st_ok = std::string(strategy) == "channel" ? (st == "channel" || st == "tensor") : st == strategy;
+    if (!st_ok) return bad(p + ".strategy", "\"" + st + "\" is not supported (" + (std::string(strategy) == "channel" ? "channel, tensor" : strategy) + ")");
+    if (a.get("dynamic").as_bool(!dynamic) != dynamic) return bad(p + ".dynamic", dynamic ? "must be true" : "must be false");
+    if (!a.get("group_size").is_null()) return bad(p + ".group_size", "is not supported");
+    if (!a.get("block_structure").is_null()) return bad(p + ".block_structure", "is not supported");
+    return true;
+  };
+  if (!check("weights", "channel", false) || !check("input_activations", "token", true)) return false;
+  bool lm_head = false;
+  for (const Json& i : q.get("ignore").items()) lm_head |= i.as_string() == "lm_head";
+  if (!lm_head) return bad("ignore", "must list lm_head (the LM head stays bf16)");
+  return true;
 }
 
 bool model_config_from_hf(const Json& hf, ModelConfig* out, std::string* err) {
@@ -92,9 +146,24 @@ bool model_config_from_hf(const Json& hf, ModelConfig* out, std::string* err) {
       return false;
     }
   }
+  const Json& qc = hf.get("quantization_config");
+  if (!qc.is_null()) {
+    if (!parse_fp8_quantization(qc, err)) return false;
+    if (m.experts > 0) { *err = "config.json: quantization_config: FP8 is not supported for mixture-of-experts models"; return false; }
+    if (m.hidden % 128 || m.ffn % 128) { *err = "config.json: quantization_config: FP8 needs hidden and intermediate_size multiples of 128"; return false; }
+    m.fp8 = true;
+  }
   m.name = "checkpoint";
   *out = m;
   return true;
+}
+
+int splitk_factor_fp8(int M, int K, int N, int target_ctas, bool strict) {
+  // an FP8 k-block holds 128 e4m3 codes in the same 128-byte row as 64 bf16: the rule sees K / 2 columns
+  return splitk_factor(M, K / 2, N, target_ctas, strict);
+}
+size_t splitk_workspace_bytes_fp8(int M, int K, int max_batch, int target_ctas, bool strict) {
+  return splitk_workspace_bytes(M, K / 2, max_batch, target_ctas, strict);
 }
 
 int splitk_factor(int M, int K, int N, int target_ctas, bool strict) {

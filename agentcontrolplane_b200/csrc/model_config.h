@@ -24,6 +24,9 @@ struct ModelConfig {
   // Llama-3.1 "llama3" RoPE frequency scaling (config.json rope_scaling); factor 0 = none
   double rope_factor = 0.0, rope_low_freq = 1.0, rope_high_freq = 4.0;
   int rope_orig_max_pos = 8192;
+  // FP8 (e4m3) QKV / O / gate-up / down projections with per-row weight and per-token activation scales
+  // (DESIGN.md §5): the `-fp8` presets; dense, single-GPU models only
+  bool fp8 = false;
   int q_dim() const { return heads * HEAD_DIM; }
   int kv_dim() const { return kv_heads * HEAD_DIM; }
   int qkv_dim() const { return q_dim() + 2 * kv_dim(); }
@@ -33,7 +36,11 @@ struct ModelConfig {
   double weight_bytes() const {
     const double mlp = 3.0 * ffn * hidden * (experts > 0 ? experts : 1) + (experts > 0 ? (double)experts * hidden : 0.0);
     double per_layer = (double)qkv_dim() * hidden + (double)hidden * q_dim() + mlp + 2.0 * hidden;
-    return 2.0 * (per_layer * layers + (double)vocab * hidden + hidden);
+    if (!fp8) return 2.0 * (per_layer * layers + (double)vocab * hidden + hidden);
+    // FP8: the four projections at one byte per weight plus one fp32 scale per output row; the rest stays bf16
+    const double proj = (double)qkv_dim() * hidden + (double)hidden * q_dim() + 3.0 * ffn * hidden;
+    const double rows = (double)qkv_dim() + hidden + 2.0 * ffn + hidden;
+    return 2.0 * ((per_layer - proj) * layers + (double)vocab * hidden + hidden) + (proj + 4.0 * rows) * layers;
   }
   double kv_bytes_per_token() const { return 2.0 * kv_dim() * 2.0 * layers; }
   // algorithmic FLOPs of one step (SURVEY.md §8d): 2 per weight per token row for the layer matrices,
@@ -60,5 +67,8 @@ void rope_inv_freq(const ModelConfig& c, float* inv64);
 int splitk_factor(int M, int K, int N, int target_ctas, bool strict_batch_invariance);
 // fp32 split-K workspace that holds the planes of ANY decode step of up to max_batch rows of a [M][K] GEMM
 size_t splitk_workspace_bytes(int M, int K, int max_batch, int target_ctas, bool strict_batch_invariance);
+// The same rule and workspace for the FP8 GEMMs, whose k-blocks hold 128 e4m3 codes (K in elements)
+int splitk_factor_fp8(int M, int K, int N, int target_ctas, bool strict_batch_invariance);
+size_t splitk_workspace_bytes_fp8(int M, int K, int max_batch, int target_ctas, bool strict_batch_invariance);
 
 }  // namespace acp

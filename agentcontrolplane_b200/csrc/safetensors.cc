@@ -36,6 +36,7 @@ bool is_file(const std::string& p) {
 size_t dtype_size(const std::string& d) {
   if (d == "BF16" || d == "F16") return 2;
   if (d == "F32") return 4;
+  if (d == "F8_E4M3") return 1;   // FP8 codes (compressed-tensors float-quantized), used verbatim
   return 0;
 }
 

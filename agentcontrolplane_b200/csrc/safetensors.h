@@ -18,7 +18,7 @@
 namespace acp {
 
 struct StTensor {
-  std::string dtype;            // "BF16" | "F16" | "F32"
+  std::string dtype;            // "BF16" | "F16" | "F32" | "F8_E4M3"
   std::vector<int64_t> shape;
   const uint8_t* data = nullptr;
   size_t nbytes = 0;

@@ -91,7 +91,8 @@ int acp_host_render_prompt_with(const char* tokenizer_path, const char* chat_req
  * acp_infer_init {"weights": dir} does and reports
  *   {"dir":…, "config":{…config.json…}, "tensors":{"name":{"dtype","shape","nbytes"}},
  *    "model":{"hidden":…, "layers":…, "heads":…, "kv_heads":…, "ffn":…, "vocab":…, "rope_theta":…,
- *             "eps":…, "tied_embeddings":…, "rope_inv_freq":[64 floats]}}
+ *             "eps":…, "tied_embeddings":…, "weight_dtype": "bf16" | "fp8_e4m3", "rope_inv_freq":[64 floats]}}
+ * A quantization_config other than compressed-tensors FP8_DYNAMIC (DESIGN.md §2) is refused with the field named.
  * or {"error": "..."} with return code ACP_ERR_INVALID. */
 int acp_host_checkpoint_index(const char* path, char** out_json);
 
@@ -99,6 +100,9 @@ int acp_host_checkpoint_index(const char* path, char** out_json);
  * out[N][M] = X[N][K] W[M][K]^T, and the workspace bytes that hold the planes of ANY step of up to max_batch rows. */
 int acp_host_splitk_factor(int M, int K, int N, int target_ctas, int strict_batch_invariance);
 size_t acp_host_splitk_workspace_bytes(int M, int K, int max_batch, int target_ctas, int strict_batch_invariance);
+/* The same for the FP8 (e4m3) GEMMs of FP8 models, whose k-blocks hold 128 codes; K in elements. */
+int acp_host_splitk_factor_fp8(int M, int K, int N, int target_ctas, int strict_batch_invariance);
+size_t acp_host_splitk_workspace_bytes_fp8(int M, int K, int max_batch, int target_ctas, int strict_batch_invariance);
 /* One tensor of the checkpoint as the bf16 bits the loader uploads (BF16 verbatim; F16 / F32 rounded
  * to nearest even).  out == NULL: only *n_elems is set.  ACP_ERR_NOT_FOUND: no such tensor. */
 int acp_host_checkpoint_tensor_bf16(const char* path, const char* name, uint16_t* out, size_t max_elems,

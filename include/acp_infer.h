@@ -49,8 +49,14 @@ typedef struct acp_engine acp_engine;
  * llmclient.NewLangchainClient (langchaingo_client.go:27-80): the Go `local` client is a
  * zero-cost handle onto this singleton.  config_json keys (all optional):
  *   "model": "llama-3-8b" | "llama-3-8b-l2" | "llama-3-70b" | "tiny" | "tiny-g2"
+ *            | "<dense single-GPU preset>-fp8" (llama-3-8b-fp8, llama-3-8b-l2-fp8, tiny-fp8, tiny-g2-fp8,
+ *              tiny-g8-fp8): the same synthetic weights with the four layer projections quantised to e4m3
+ *              (per-row weight scales, per-token activation scales; DESIGN.md §5); acp_infer_stats reports
+ *              "weight_dtype"
  *   "weights": "synthetic" (seeded generator, default) | "<dir>" = HuggingFace Llama checkpoint
  *              (config.json + model.safetensors or model.safetensors.index.json + shards; BF16/F16/F32;
+ *              or compressed-tensors FP8_DYNAMIC: F8_E4M3 projections with per-channel or per-tensor
+ *              weight_scale, served on the FP8 GEMMs, one GPU; DESIGN.md §2;
  *              "model" is then just the name requests must carry, default = the directory name)
  *   "seed": 11317760                  (0xACB200)
  *   "device": 0, "max_batch": 256, "max_tokens_per_step": 8192, "kv_pages": 2048,

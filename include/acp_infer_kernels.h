@@ -32,6 +32,21 @@ int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int N, int K, i
                     int epi, int bn, void* out, float* amax_val, int* amax_idx, int iters,
                     float* elapsed_ms);
 
+/* FP8 (e4m3) GEMM of the `-fp8` presets: w = e4m3 codes [M][K] with fp32 scales w_scale[M], x = e4m3
+ * codes [N][K] with fp32 scales x_scale[N]; out[n][m] = fp32(fp32(acc * w_scale[m]) * x_scale[n]) with
+ * acc = sum_k w[m][k] * x[n][k] (DESIGN.md §5), then stored as for acp_kernel_gemm: epi 0 bf16 [N][M],
+ * epi 1 fp32 [splits][N][M] (each split scaled), epi 3 SwiGLU bf16 [N][M/2] (gate and up rows scaled by
+ * their own w_scale before the bf16 rounding).  No arg-max epilogue.  bn = 0 picks the N tile from N;
+ * otherwise 16..128; bn = -1 (N > 256, epi 0, 1 or 3) forces the persistent prefill kernel.  iters > 0
+ * also stores the mean milliseconds of `iters` launches (L2 flushed between launches) in *elapsed_ms. */
+int acp_kernel_gemm_fp8(const uint8_t* w, const float* w_scale, const uint8_t* x, const float* x_scale, int M, int N,
+                        int K, int splits, int epi, int bn, void* out, int iters, float* elapsed_ms);
+
+/* The FP8 row quantiser on the device: x = bf16 bit patterns [rows][cols] (cols % 8 == 0) ->
+ * codes = e4m3 [rows][cols], scales = fp32 [rows]; amax = max|x|, s = fp32(amax / 448) (1 for a zero
+ * row), code = e4m3_rne(clamp(fp32(x / s), -448, 448)). */
+int acp_kernel_quantize_fp8(const uint16_t* x, int rows, int cols, uint8_t* codes, float* scales);
+
 /* Causal paged-KV GQA attention of ONE sequence's prefill chunk.  q: bf16 [q_len][heads][128] (already
  * rotated), k, v: bf16 [ctx][kv_heads][128] — the whole context, the last q_len keys belong to the
  * query tokens (query i sits at absolute position ctx - q_len + i and sees keys 0..that position).
