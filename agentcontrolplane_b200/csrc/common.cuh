@@ -123,6 +123,36 @@ ACP_DEVINL void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
 ACP_DEVINL void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// ---------------------------------------------------------------------------------
+// thread-block clusters
+// ---------------------------------------------------------------------------------
+ACP_DEVINL uint32_t cluster_ctarank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster (release / acquire: memory operations before it are visible to
+// the peers after it; a release at cluster scope costs a MEMBAR.GPU, so this is for kernel exit)
+ACP_DEVINL void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// the same without the release: after mbarrier initialisation, which fence_mbar_init() already publishes
+// to the cluster
+ACP_DEVINL void cluster_sync_relaxed() {
+  asm volatile("barrier.cluster.arrive.relaxed;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
+}
+// arrive on the mbarrier at the same shared-memory offset in CTA `rank` of the cluster.  Default semantics
+// (release at CTA scope), like the local mbar_arrive: a cluster-scope release would put a MEMBAR.GPU in front
+// of every arrival, and what the arrival orders (wgmma reads of a stage before the peer's TMA refills it) is
+// ordered by the mbarrier itself.
+ACP_DEVINL void mbar_arrive_cluster(uint64_t* bar, uint32_t rank) {
+  asm volatile(
+      "{\n\t.reg .b32 ra;\n\t"
+      "mapa.shared::cluster.u32 ra, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [ra];\n\t}"
+      ::"r"(smem_u32(bar)), "r"(rank)
+      : "memory");
+}
 ACP_DEVINL bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
   uint32_t ok;
   asm volatile(
@@ -193,6 +223,36 @@ ACP_DEVINL void tma_load_2d(void* smem_dst, const void* tmap, uint64_t* bar, int
       :
       : "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
+}
+// The same load multicast to the CTAs of `cta_mask` in the cluster: the box lands at the same CTA-relative
+// shared-memory offset in each of them and completes on the mbarrier at the same offset in each.
+ACP_DEVINL void tma_load_2d_multicast(void* smem_dst, const void* tmap, uint64_t* bar, int c0, int c1, uint16_t cta_mask,
+                                      uint64_t hint) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster.L2::cache_hint"
+      " [%0], [%1, {%3, %4}], [%2], %5, %6;"
+      :
+      : "r"(smem_u32(smem_dst)), "l"(tmap), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "h"(cta_mask), "l"(hint)
+      : "memory");
+}
+// four 8x8 b16 matrices from registers (accumulator-fragment layout: lane l holds row l/4, columns 2(l%4),
+// 2(l%4)+1 of each) to shared memory TRANSPOSED: lane 8i + k gives the address of row k of matrix i's
+// transpose, i.e. the 8 elements of column k, stored as 16 contiguous bytes.
+ACP_DEVINL void stmatrix_x4_trans(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.trans.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
+// shared-memory accesses by 32-bit shared-window address (the generic-pointer forms cost 64-bit registers)
+ACP_DEVINL void sts_u16(uint32_t addr, uint16_t v) { asm volatile("st.shared.u16 [%0], %1;" ::"r"(addr), "h"(v) : "memory"); }
+ACP_DEVINL uint4 lds_v4(uint32_t addr) {
+  uint4 v;
+  asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+  return v;
+}
+// named barrier over `threads` threads (ids 0 = __syncthreads, 1 = the GEMM's 8 consumer warps)
+ACP_DEVINL void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 // 1D bulk copy global -> shared (no tensor map), completes on an mbarrier.
 ACP_DEVINL void bulk_load_1d(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {

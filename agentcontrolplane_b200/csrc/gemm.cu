@@ -170,6 +170,10 @@ int gemm_path(const GemmLaunch& g) {
   return GEMM_PATH_TILED;
 }
 
+// Co-resident 2-CTA clusters of each persistent instantiation ([FP8][EPI]), from cudaOccupancyMaxActiveClusters
+// in gemm_setup_attributes (0 until then).
+static int g_pgemm_clusters[2][4] = {};
+
 template <int EPI, bool FP8 = false>
 static int launch_persistent(const GemmLaunch& g, cudaStream_t stream) {
   constexpr int BN = FP8 ? PGEMM_BN_E4M3 : PGEMM_BN;
@@ -179,10 +183,27 @@ static int launch_persistent(const GemmLaunch& g, cudaStream_t stream) {
   a.group_ranges = nullptr;
   a.w_scale = g.w_scale; a.x_scale = g.x_scale;
   const int m_tiles = (g.M + GEMM_BM - 1) / GEMM_BM, n_tiles = (g.N + BN - 1) / BN;
-  int grid = m_tiles * n_tiles;
-  if (grid > GEMM_SMS) grid = GEMM_SMS;  // one persistent CTA per SM
-  cudaError_t e = acp_launch(gemm_wx_persistent_kernel<EPI, FP8>, dim3(grid), dim3(GEMM_THREADS), GemmCfg<BN>::kSmemBytes, stream,
-                             *g.w, g.x->x[FP8 ? 3 : 4], a, m_tiles, n_tiles);
+  const int max_clusters = g_pgemm_clusters[FP8][EPI];
+  if (max_clusters <= 0) {
+    fprintf(stderr, "[acp_infer] persistent gemm: no co-resident cluster count (gemm_setup_attributes not run)\n");
+    return -5;
+  }
+  int clusters = ((m_tiles + 1) / 2) * n_tiles;   // one cluster per pair of m-tiles of an n-tile
+  if (clusters > max_clusters) clusters = max_clusters;
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2 * clusters);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = PGemmSmem<FP8>;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[2];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = acp_pdl_enabled() ? 2 : 1;
+  // X in halves of BN / 2 token rows, one per CTA of the cluster (box 128 rows for bf16, 64 for FP8)
+  cudaError_t e = cudaLaunchKernelEx(&cfg, gemm_wx_persistent_kernel<EPI, FP8>, *g.w, g.x->x[FP8 ? 2 : 3], a, m_tiles, n_tiles);
   if (e != cudaSuccess) {
     fprintf(stderr, "[acp_infer] persistent gemm launch failed EPI=%d: %s\n", EPI, cudaGetErrorString(e));
     return -5;
@@ -240,9 +261,30 @@ static int set_attr_bn() {
 }
 template <int EPI, bool FP8>
 static int set_attr_persistent() {
-  constexpr int bytes = GemmCfg<FP8 ? PGEMM_BN_E4M3 : PGEMM_BN>::kSmemBytes;
-  return cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) == cudaSuccess ? 0 : -5;
+  constexpr int bytes = PGemmSmem<FP8>;
+  if (cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
+    return -5;
+  // how many 2-CTA clusters of this kernel fit on the device at once (the persistent grid)
+  cudaLaunchConfig_t cfg = {};
+  cfg.gridDim = dim3(2 * GEMM_SMS);
+  cfg.blockDim = dim3(GEMM_THREADS);
+  cfg.dynamicSmemBytes = bytes;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeClusterDimension;
+  attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  int clusters = 0;
+  cudaError_t e = cudaOccupancyMaxActiveClusters(&clusters, gemm_wx_persistent_kernel<EPI, FP8>, &cfg);
+  if (e != cudaSuccess || clusters <= 0) {
+    fprintf(stderr, "[acp_infer] cudaOccupancyMaxActiveClusters(persistent gemm EPI=%d FP8=%d) = %d: %s\n", EPI, (int)FP8, clusters,
+            cudaGetErrorString(e));
+    return -5;
+  }
+  g_pgemm_clusters[FP8][EPI] = clusters;
+  return 0;
 }
+int gemm_persistent_clusters(bool fp8, int epi) { return (epi >= 0 && epi < 4) ? g_pgemm_clusters[fp8][epi] : 0; }
 int gemm_setup_attributes() {
   int rc = set_attr_bn<16>() | set_attr_bn<32>() | set_attr_bn<64>() | set_attr_bn<128>() |
            set_attr_bn<256>();

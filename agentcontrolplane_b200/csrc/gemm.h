@@ -61,5 +61,7 @@ int gemm_launch(const GemmLaunch& g, cudaStream_t stream);
 enum { GEMM_PATH_TILED = 0, GEMM_PATH_PERSISTENT = 1 };
 int gemm_path(const GemmLaunch& g);   // the kernel gemm_launch would pick for this problem
 int gemm_setup_attributes();  // cudaFuncSetAttribute for every instantiation (once per device)
+// co-resident 2-CTA clusters of the persistent kernel (its grid is twice that), set by gemm_setup_attributes
+int gemm_persistent_clusters(bool fp8, int epi);
 
 }  // namespace acp

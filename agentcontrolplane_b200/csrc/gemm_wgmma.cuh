@@ -19,9 +19,13 @@
 // summed IN FIXED ORDER by the consumer kernel (rope / add+rmsnorm / swiglu), which keeps the
 // result bit-reproducible run to run (no atomics).
 //
-// Persistent flavour (prefill, N > 256): one CTA per SM walks (m-tile, 256-token n-tile) tiles; the
-// producer streams the next tile's stages while the consumers run the previous tile's epilogue.
-// Both flavours accumulate K in the same order, so they agree bit for bit.
+// Persistent flavour (prefill, N > 256): 2-CTA clusters, one CTA per SM, walk pairs of m-tiles of one
+// 256-token n-tile; each CTA loads its own weight tile and half of the activation tile, TMA-multicast to both
+// (each CTA reads 32 KiB from L2 per 64-wide k-block instead of 48: W 16 + its X half 16).  The
+// producer streams the next tile's stages while the consumers run the previous tile's epilogue, which for
+// bf16 and SwiGLU outputs goes through a per-warpgroup shared-memory staging buffer (stmatrix .trans) and
+// leaves as 16-byte row pieces.  Both flavours accumulate K in the same order and round the same way, so
+// they agree bit for bit.
 //
 // FP8 flavour (template flag FP8, the `-fp8` presets): W and X hold e4m3 codes, a k-block is still one
 // 128-byte swizzle row (now 128 elements) and a tile still 128 rows x 128 B, so the ring is unchanged;
@@ -92,6 +96,11 @@ constexpr int PGEMM_BN = 256;
 using PGemmCfg = GemmCfg<PGEMM_BN>;
 constexpr int GEMM_BK_E4M3 = 128;   // e4m3 elements per k-block (the same 128-byte swizzle row)
 constexpr int PGEMM_BN_E4M3 = 128;
+constexpr int PGEMM_STAGE_BYTES = 16384;   // epilogue staging buffer per consumer warpgroup (persistent kernel)
+// dynamic shared memory of the persistent kernel: ring, barriers (<= 256 B), then the two staging buffers
+// (bf16: 4 x 48 KiB + 32 KiB + 1.25 KiB = 225.25 KiB of the 227 KiB an SM allows)
+template <bool FP8>
+constexpr int PGemmSmem = GemmCfg<FP8 ? PGEMM_BN_E4M3 : PGEMM_BN>::kSmemBytes + 2 * PGEMM_STAGE_BYTES;
 
 // ---------------------------------------------------------------------------------
 // producer: the k-blocks [kb_begin, kb_end) of one tile into the ring (one thread)
@@ -111,13 +120,43 @@ __device__ __forceinline__ void gemm_produce(uint8_t* smem, uint64_t* full_bar, 
   }
 }
 
+// Producer of one CTA of a 2-CTA cluster (persistent kernel): the two CTAs work on m-tiles 2p, 2p+1 of the
+// same n-tile.  Each loads its own W tile and half of the X box (BN/2 token rows, `rank` picks the half),
+// multicast to both CTAs at the same offset, so every stage still holds W + the whole X tile.  A stage is
+// refilled once the consumers of BOTH CTAs have released it (the empty barriers count 16 warps).  `has_w`
+// false: the second CTA of a last, odd m-tile has no W tile; it still loads its X half, and expects only X.
+template <int BN, int STAGES, int BK>
+__device__ __forceinline__ void gemm_produce_pair(uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar, int& s, uint32_t& ph,
+                                                  const CUtensorMap* tmap_w, const CUtensorMap* tmap_xh, int w_row0, bool has_w,
+                                                  int nkb, int x_row, uint32_t rank) {
+  using Cfg = GemmCfg<BN>;
+  constexpr int kHalfBytes = Cfg::kBBytes / 2;
+  for (int kb = 0; kb < nkb; ++kb) {
+    mbar_wait_mma(&empty_bar[s], ph ^ 1);
+    uint8_t* a_dst = smem + s * Cfg::kStageBytes;
+    mbar_arrive_expect_tx(&full_bar[s], has_w ? Cfg::kStageBytes : Cfg::kBBytes);
+    if (has_w) tma_load_2d(a_dst, tmap_w, &full_bar[s], 0, w_row0 + kb * GEMM_BM, kEvictNormal);
+    tma_load_2d_multicast(a_dst + Cfg::kABytes + rank * kHalfBytes, tmap_xh, &full_bar[s], kb * BK, x_row + (int)rank * (BN / 2),
+                          0x3, kEvictNormal);
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+}
+
+// A consumer warp releases stage `bar`: its own CTA's empty barrier, and with PAIR also the cluster peer's
+// (rank ^ 1), whose producer multicasts into this CTA's stages too.
+template <bool PAIR>
+__device__ __forceinline__ void gemm_release(uint64_t* bar, uint32_t rank) {
+  mbar_arrive(bar);
+  if constexpr (PAIR) mbar_arrive_cluster(bar, rank ^ 1u);
+}
+
 // ---------------------------------------------------------------------------------
 // consumer warpgroup `wg` (0/1): d = W[rows 64*wg ..][k-blocks] x X^T over nkb ring stages.
-// Every warp releases a stage once its own MMAs have read it (empty barriers count 8 warps).
+// Every warp releases a stage once its own MMAs have read it (empty barriers count 8 warps, 16 with PAIR).
 // ---------------------------------------------------------------------------------
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool PAIR = false>
 __device__ __forceinline__ void gemm_consume(float (&d)[BN / 2], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                             int& s, uint32_t& ph, int nkb, int wg, int lane) {
+                                             int& s, uint32_t& ph, int nkb, int wg, int lane, uint32_t rank = 0) {
   using Cfg = GemmCfg<BN>;
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
@@ -134,20 +173,20 @@ __device__ __forceinline__ void gemm_consume(float (&d)[BN / 2], uint8_t* smem, 
       wgmma_bf16_ss<BN>(d, a_desc + (uint64_t)(k * 2), b_desc + (uint64_t)(k * 2), (kb > 0 || k > 0) ? 1u : 0u);
     wgmma_commit();
     wgmma_wait<1>();   // the MMAs of the previous stage are done: release it
-    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+    if (prev >= 0 && lane == 0) gemm_release<PAIR>(&empty_bar[prev], rank);
     prev = s;
     if (++s == STAGES) { s = 0; ph ^= 1; }
   }
   wgmma_wait<0>();
   wgmma_fence_regs(d);
-  if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+  if (prev >= 0 && lane == 0) gemm_release<PAIR>(&empty_bar[prev], rank);
 }
 
 // FP8 consumer: per k-block, four k32 MMAs into the scratch accumulator t (the first overwrites it), then
 // d += t in fp32 once they are done.  The stage is released right after the wait, before the adds.
-template <int BN, int STAGES>
+template <int BN, int STAGES, bool PAIR = false>
 __device__ __forceinline__ void gemm_consume_e4m3(float (&d)[BN / 2], uint8_t* smem, uint64_t* full_bar, uint64_t* empty_bar,
-                                                  int& s, uint32_t& ph, int nkb, int wg, int lane) {
+                                                  int& s, uint32_t& ph, int nkb, int wg, int lane, uint32_t rank = 0) {
   using Cfg = GemmCfg<BN>;
   float t[BN / 2];
 #pragma unroll
@@ -165,7 +204,7 @@ __device__ __forceinline__ void gemm_consume_e4m3(float (&d)[BN / 2], uint8_t* s
     wgmma_commit();
     wgmma_wait<0>();
     wgmma_fence_regs(t);
-    if (lane == 0) mbar_arrive(&empty_bar[s]);
+    if (lane == 0) gemm_release<PAIR>(&empty_bar[s], rank);
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) d[i] += t[i];
     if (++s == STAGES) { s = 0; ph ^= 1; }
@@ -232,6 +271,88 @@ __device__ __forceinline__ void gemm_store(const float (&d)[BN / 2], const GemmA
         out[(size_t)n * args.ld + (m >> 1)] = __float2bfloat16_rn(act * u);
       }
     }
+  }
+}
+
+// ---------------------------------------------------------------------------------
+// persistent-kernel epilogue through shared memory (bf16 and SwiGLU outputs): each consumer warpgroup writes
+// its 64 output features x BN tokens into its own 16 KiB staging buffer, then stores 16-byte pieces of output
+// rows.  Every value and rounding is the one gemm_store computes; only the way it reaches global memory
+// differs (from registers each warp store touches 4-8 rows with 2 bytes per lane).  Staging rows are 16-byte
+// chunks XOR-swizzled by the row index so that both the writes and the row reads are free of bank conflicts.
+// `tid` = thread in the warpgroup (0..127), `w4` = warp in the warpgroup.
+// ---------------------------------------------------------------------------------
+// one staged piece of 8 outputs, columns [col, col + 8) of an output row: one 16-byte store, or element by
+// element where the piece runs past the last column (ragged M) or rows are not 16-byte aligned (!vec_ok)
+__device__ __forceinline__ void gemm_store_piece(__nv_bfloat16* row, int col, int ncols, bool vec_ok, uint32_t src) {
+  const uint4 v = lds_v4(src);
+  if (vec_ok && col + 8 <= ncols) {
+    *(uint4*)(row + col) = v;
+  } else {
+    const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+    for (int q = 0; q < 8; ++q)
+      if (col + q < ncols) row[col + q] = __ushort_as_bfloat16((unsigned short)(w[q >> 1] >> (16 * (q & 1))));
+  }
+}
+// bf16: rows of 64 features (128 B) per token, 128 tokens per pass (stmatrix .trans turns the [m][n]
+// accumulator fragments into [n][m] rows)
+template <int BN>
+__device__ __forceinline__ void gemm_store_staged_bf16(const float (&d)[BN / 2], const GemmArgs& args, uint8_t* stage, int m_wg0,
+                                                       int n0, int n_valid, bool vec_ok, int wg, int w4, int lane, int tid) {
+  constexpr int PASS_N = PGEMM_STAGE_BYTES / 128;
+  const uint32_t st = smem_u32(stage);
+  __nv_bfloat16* out = (__nv_bfloat16*)args.out;
+#pragma unroll
+  for (int p = 0; p < BN / PASS_N + (BN < PASS_N ? 1 : 0); ++p) {
+    named_bar_sync(2 + wg, 128);   // the previous pass (or tile) has read the buffer
+#pragma unroll
+    for (int j = p * PASS_N / 8; j < (p + 1) * PASS_N / 8 && j < BN / 8; j += 2) {
+      // matrices (features 8h.., tokens 8j'..) for h = i & 1, j' = j + (i >> 1); this lane addresses token row k
+      const int i = lane >> 3, k = lane & 7;
+      const int n = 8 * (j - p * PASS_N / 8 + (i >> 1)) + k, c = 2 * w4 + (i & 1);
+      stmatrix_x4_trans(st + n * 128 + ((c ^ (n & 7)) << 4), pack_bf16x2(d[4 * j], d[4 * j + 1]),
+                        pack_bf16x2(d[4 * j + 2], d[4 * j + 3]), pack_bf16x2(d[4 * j + 4], d[4 * j + 5]),
+                        pack_bf16x2(d[4 * j + 6], d[4 * j + 7]));
+    }
+    named_bar_sync(2 + wg, 128);
+    constexpr int ROWS = BN < PASS_N ? BN : PASS_N;
+#pragma unroll
+    for (int it = 0; it < ROWS * 8 / 128; ++it) {
+      const int idx = it * 128 + tid, n = idx >> 3, c = idx & 7, gn = n0 + p * PASS_N + n;
+      if (gn < n_valid)
+        gemm_store_piece(out + (size_t)gn * args.ld, m_wg0 + 8 * c, args.M, vec_ok, st + n * 128 + ((c ^ (n & 7)) << 4));
+    }
+  }
+}
+
+// SwiGLU: rows of 32 outputs (64 B) per token, the whole tile in one pass; the arithmetic is gemm_store's
+template <int BN>
+__device__ __forceinline__ void gemm_store_staged_swiglu(const float (&d)[BN / 2], const GemmArgs& args, uint8_t* stage, int m_wg0,
+                                                         int n0, int n_valid, bool vec_ok, int wg, int w4, int lane, int tid) {
+  static_assert(BN * 64 <= PGEMM_STAGE_BYTES, "one pass");
+  const uint32_t st = smem_u32(stage);
+  const bool odd = (lane >> 2) & 1;
+  named_bar_sync(2 + wg, 128);
+#pragma unroll
+  for (int i = 0; i < BN / 2; i += 2) {
+    const float mine0 = bf16_round(d[i]);
+    const float mine1 = bf16_round(d[i + 1]);
+    const float got = __shfl_xor_sync(0xffffffffu, odd ? mine0 : mine1, 4);
+    const float g = odd ? got : mine0;
+    const float u = odd ? mine1 : got;
+    const float act = bf16_round(g / (1.0f + expf(-g)));
+    const int col = (16 * w4 + (lane >> 2) + 8 * ((i >> 1) & 1)) >> 1;          // output column in the warpgroup
+    const int n = 2 * (lane & 3) + 8 * (i >> 2) + (odd ? 1 : 0);                 // token in the tile
+    sts_u16(st + n * 64 + (((col >> 3) ^ ((n >> 1) & 3)) << 4) + (col & 7) * 2, f32_to_bf16_bits(act * u));
+  }
+  named_bar_sync(2 + wg, 128);
+  __nv_bfloat16* out = (__nv_bfloat16*)args.out;
+#pragma unroll
+  for (int it = 0; it < BN * 4 / 128; ++it) {
+    const int idx = it * 128 + tid, n = idx >> 2, c = idx & 3, gn = n0 + n;
+    if (gn < n_valid)
+      gemm_store_piece(out + (size_t)gn * args.ld, (m_wg0 >> 1) + 8 * c, args.M >> 1, vec_ok, st + n * 64 + ((c ^ ((n >> 1) & 3)) << 4));
   }
 }
 
@@ -384,59 +505,77 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
   }
 }
 
-// Persistent kernel (prefill): grid = min(tiles, SMs); tile t = (m-tile t / n_tiles, n-tile t % n_tiles),
-// n-tile fastest (CTAs running together share a weight tile; X stays in L2).  bf16, SwiGLU or one fp32 plane.
+// Persistent kernel (prefill), launched as 2-CTA clusters: grid = 2 x min(tile pairs, co-resident clusters).
+// Pair p = (m-tiles 2(p / n_tiles) and 2(p / n_tiles) + 1, n-tile p % n_tiles), n-tile fastest (clusters
+// running together share weight tiles; X stays in L2); cluster CTA `rank` takes m-tile 2(p / n_tiles) + rank.
+// Both CTAs walk the same pairs in lockstep, so their rings advance stage for stage: each loads its own W
+// tile and multicasts half of the X tile to both (`tmap_xh`: a box of BN/2 token rows; gemm_produce_pair).
+// bf16, SwiGLU or one fp32 plane.
 template <int EPI, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
-gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_x,
+gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_xh,
                           GemmArgs args, int m_tiles, int n_tiles) {
   constexpr int BN = FP8 ? PGEMM_BN_E4M3 : PGEMM_BN;
   using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::kStages;
   constexpr int BK = FP8 ? GEMM_BK_E4M3 : GEMM_BK;
   extern __shared__ uint8_t smem_raw[];
+  // the same alignment in both CTAs of the cluster (the dynamic shared window starts at the same offset), so
+  // a multicast box lands at the same offset of the ring in each
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const uint32_t rank = cluster_ctarank();
+  const int cluster = (int)blockIdx.x >> 1, clusters = (int)gridDim.x >> 1;
   const int nkb = (args.K + BK - 1) / BK;
-  const int num_tiles = m_tiles * n_tiles;
+  const int num_pairs = ((m_tiles + 1) >> 1) * n_tiles;
 
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_w);
-    tma_prefetch_desc(&tmap_x);
-    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    tma_prefetch_desc(&tmap_xh);
+    for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 16); }
     fence_mbar_init();
   }
-  __syncthreads();
+  cluster_sync_relaxed();   // both CTAs' barriers are initialised before either multicasts or arrives on them
 
   int s = 0;
   uint32_t ph = 0;
   if (warp < 4) {
     if (threadIdx.x == 0) {
       pdl_wait();  // activations come from the previous kernel
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x)
-        gemm_produce<BN, STAGES, BK>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_x, (t / n_tiles) * nkb * GEMM_BM, 0, nkb,
-                                 (t % n_tiles) * BN, kEvictNormal);
+      for (int p = cluster; p < num_pairs; p += clusters) {
+        const int m_tile = 2 * (p / n_tiles) + (int)rank;
+        gemm_produce_pair<BN, STAGES, BK>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_xh, m_tile * nkb * GEMM_BM,
+                                          m_tile < m_tiles, nkb, (p % n_tiles) * BN, rank);
+      }
     }
   } else {
-    const int wg = (warp >> 2) - 1, cw = warp - 4;
+    const int wg = (warp >> 2) - 1, cw = warp - 4, tid = threadIdx.x & 127;
+    uint8_t* stage = (uint8_t*)(empty_bar + STAGES) + wg * PGEMM_STAGE_BYTES;   // PGemmSmem: past the barriers
+    // 16-byte stores need output rows that start 16-byte aligned
+    const bool vec_ok = args.ld % 8 == 0 && ((uintptr_t)args.out & 15) == 0;
     pdl_wait();
     const int n_valid = args.n_dev ? *args.n_dev : args.N;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
+    for (int p = cluster; p < num_pairs; p += clusters) {
+      const int m_tile = 2 * (p / n_tiles) + (int)rank, m_base = m_tile * GEMM_BM + cw * 16, n0 = (p % n_tiles) * BN;
       float d[BN / 2];
-      if constexpr (FP8) {
-        gemm_consume_e4m3<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
-        gemm_scale_e4m3<BN>(d, args, (t / n_tiles) * GEMM_BM + cw * 16, (t % n_tiles) * BN, 0, n_valid, lane);
-      } else {
-        gemm_consume<BN, STAGES>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane);
+      // a CTA without a W tile still consumes (and releases) every stage: its peer's X half needs the slot
+      if constexpr (FP8) gemm_consume_e4m3<BN, STAGES, true>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane, rank);
+      else gemm_consume<BN, STAGES, true>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane, rank);
+      if (m_tile < m_tiles) {
+        if constexpr (FP8) gemm_scale_e4m3<BN>(d, args, m_base, n0, 0, n_valid, lane);
+        const int m_wg0 = m_tile * GEMM_BM + 64 * wg;
+        if constexpr (EPI == EPI_BF16) gemm_store_staged_bf16<BN>(d, args, stage, m_wg0, n0, n_valid, vec_ok, wg, cw & 3, lane, tid);
+        else if constexpr (EPI == EPI_SWIGLU) gemm_store_staged_swiglu<BN>(d, args, stage, m_wg0, n0, n_valid, vec_ok, wg, cw & 3, lane, tid);
+        else gemm_store<BN, EPI>(d, args, m_base, n0, 0, n_valid, 0, lane);   // the fp32 plane, from registers
       }
-      gemm_store<BN, EPI>(d, args, (t / n_tiles) * GEMM_BM + cw * 16, (t % n_tiles) * BN, 0, n_valid, 0, lane);
     }
   }
+  cluster_sync();   // no CTA exits while its peer may still multicast into it or arrive on its barriers
 }
 
 }  // namespace acp

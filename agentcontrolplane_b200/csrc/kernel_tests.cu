@@ -37,6 +37,11 @@ extern "C" int acp_kernel_gemm_path(int M, int N, int K, int splits, int epi, in
   return gemm_path(g);
 }
 
+extern "C" int acp_kernel_gemm_persistent_clusters(int fp8, int epi) {
+  if (acp_kernel_device_count() <= 0 || gemm_setup_attributes() != 0) return -5;
+  return gemm_persistent_clusters(fp8 != 0, epi);
+}
+
 extern "C" int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int N, int K,
                                int splits, int epi, int bn, void* out, float* amax_val,
                                int* amax_idx, int iters, float* elapsed_ms) {

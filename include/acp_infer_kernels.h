@@ -27,6 +27,9 @@ extern "C" {
 /* Which kernel the dispatcher picks for this problem (host logic only, no GPU needed): 0 = tiled
  * gemm_wx_kernel, 1 = persistent kernel.  `splits`, `epi` and `bn` as below. */
 int acp_kernel_gemm_path(int M, int N, int K, int splits, int epi, int bn);
+/* 2-CTA clusters the persistent prefill GEMM launches (bf16 or FP8 flavour, epilogue epi): what
+   cudaOccupancyMaxActiveClusters reports for it on the current device; < 0 on error. */
+int acp_kernel_gemm_persistent_clusters(int fp8, int epi);
 
 int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int N, int K, int splits,
                     int epi, int bn, void* out, float* amax_val, int* amax_idx, int iters,
