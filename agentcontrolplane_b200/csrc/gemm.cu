@@ -193,7 +193,7 @@ static int launch_persistent(const GemmLaunch& g, cudaStream_t stream) {
   cudaLaunchConfig_t cfg = {};
   cfg.gridDim = dim3(2 * clusters);
   cfg.blockDim = dim3(GEMM_THREADS);
-  cfg.dynamicSmemBytes = PGemmSmem<FP8>;
+  cfg.dynamicSmemBytes = PGemmSmem<EPI, FP8>;
   cfg.stream = stream;
   cudaLaunchAttribute attr[2];
   attr[0].id = cudaLaunchAttributeClusterDimension;
@@ -261,7 +261,7 @@ static int set_attr_bn() {
 }
 template <int EPI, bool FP8>
 static int set_attr_persistent() {
-  constexpr int bytes = PGemmSmem<FP8>;
+  constexpr int bytes = PGemmSmem<EPI, FP8>;
   if (cudaFuncSetAttribute(gemm_wx_persistent_kernel<EPI, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes) != cudaSuccess)
     return -5;
   // how many 2-CTA clusters of this kernel fit on the device at once (the persistent grid)

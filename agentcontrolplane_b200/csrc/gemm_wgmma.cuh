@@ -21,11 +21,11 @@
 //
 // Persistent flavour (prefill, N > 256): 2-CTA clusters, one CTA per SM, walk pairs of m-tiles of one
 // 256-token n-tile; each CTA loads its own weight tile and half of the activation tile, TMA-multicast to both
-// (each CTA reads 32 KiB from L2 per 64-wide k-block instead of 48: W 16 + its X half 16).  The
-// producer streams the next tile's stages while the consumers run the previous tile's epilogue, which for
-// bf16 and SwiGLU outputs goes through a per-warpgroup shared-memory staging buffer (stmatrix .trans) and
-// leaves as 16-byte row pieces.  Both flavours accumulate K in the same order and round the same way, so
-// they agree bit for bit.
+// (each CTA reads 32 KiB from L2 per 64-wide k-block instead of 48: W 16 + its X half 16).  For bf16 and
+// SwiGLU outputs the consumers only write the finished tile, bf16-rounded, into a whole-tile shared-memory
+// staging buffer (stmatrix .trans) and go on to the next tile's MMAs; warps 1-3 of warpgroup 0 (the
+// epilogue role) read it back, apply SwiGLU, and store 16-byte row pieces while that mainloop runs.  Both
+// flavours accumulate K in the same order and round the same way, so they agree bit for bit.
 //
 // FP8 flavour (template flag FP8, the `-fp8` presets): W and X hold e4m3 codes, a k-block is still one
 // 128-byte swizzle row (now 128 elements) and a tile still 128 rows x 128 B, so the ring is unchanged;
@@ -96,11 +96,21 @@ constexpr int PGEMM_BN = 256;
 using PGemmCfg = GemmCfg<PGEMM_BN>;
 constexpr int GEMM_BK_E4M3 = 128;   // e4m3 elements per k-block (the same 128-byte swizzle row)
 constexpr int PGEMM_BN_E4M3 = 128;
-constexpr int PGEMM_STAGE_BYTES = 16384;   // epilogue staging buffer per consumer warpgroup (persistent kernel)
-// dynamic shared memory of the persistent kernel: ring, barriers (<= 256 B), then the two staging buffers
-// (bf16: 4 x 48 KiB + 32 KiB + 1.25 KiB = 225.25 KiB of the 227 KiB an SM allows)
-template <bool FP8>
-constexpr int PGemmSmem = GemmCfg<FP8 ? PGEMM_BN_E4M3 : PGEMM_BN>::kSmemBytes + 2 * PGEMM_STAGE_BYTES;
+constexpr int PGEMM_EPI_THREADS = 96;   // the epilogue role of the persistent kernel: warps 1-3 of warpgroup 0
+// Persistent kernel, per instantiation: ring depth and the whole-tile staging buffer (128 features x BN tokens
+// of bf16, one [token][64 features] half per consumer warpgroup).  The fp32 plane is stored from registers and
+// has no buffer.  Dynamic shared memory = ring, barriers (<= 256 B), staging buffer, of the 227 KiB an SM allows:
+//   bf16 / SwiGLU  3 x 48 KiB + 64 KiB + 1.25 KiB = 209.25 KiB   (a 4th stage would not fit beside the buffer)
+//   FP8            6 x 32 KiB + 32 KiB + 1.25 KiB = 225.25 KiB
+//   fp32 plane     the tiled kernel's ring (4 stages bf16, 6 FP8), no buffer
+template <int EPI, bool FP8>
+constexpr int PGemmStages = (EPI == EPI_F32 || FP8) ? GemmCfg<FP8 ? PGEMM_BN_E4M3 : PGEMM_BN>::kStages : 3;
+template <int EPI, bool FP8>
+constexpr int PGemmStagingBytes = EPI == EPI_F32 ? 0 : GEMM_BM * (FP8 ? PGEMM_BN_E4M3 : PGEMM_BN) * 2;
+template <int EPI, bool FP8>
+constexpr int PGemmSmem = PGemmStages<EPI, FP8> * GemmCfg<FP8 ? PGEMM_BN_E4M3 : PGEMM_BN>::kStageBytes + 1024 /*align*/ +
+                          256 /*barriers*/ + PGemmStagingBytes<EPI, FP8>;
+static_assert(PGemmSmem<EPI_BF16, false> <= 227 * 1024 && PGemmSmem<EPI_SWIGLU, true> <= 227 * 1024, "persistent GEMM smem");
 
 // ---------------------------------------------------------------------------------
 // producer: the k-blocks [kb_begin, kb_end) of one tile into the ring (one thread)
@@ -228,6 +238,13 @@ __device__ __forceinline__ void gemm_scale_e4m3(float (&d)[BN / 2], const GemmAr
   }
 }
 
+// bf16(bf16(silu(g)) * u) of one (gate, up) pair, g and u already bf16-rounded: the one SwiGLU expression of
+// both kernels (accurate expf and IEEE division; DESIGN.md §5)
+__device__ __forceinline__ uint16_t swiglu_bf16_bits(float g, float u) {
+  const float act = bf16_round(g / (1.0f + expf(-g)));
+  return f32_to_bf16_bits(act * u);
+}
+
 // ---------------------------------------------------------------------------------
 // epilogue from the accumulator registers (layout: common.cuh, above wgmma_bf16_ss).
 //   row m = m_base + l/4 + 8h (m_base = m0 + 64*wg + 16*warp), column n = n0 + 8j + 2(l%4) + e,
@@ -266,26 +283,25 @@ __device__ __forceinline__ void gemm_store(const float (&d)[BN / 2], const GemmA
       const float g = odd ? got : mine0;     // up lane: partner's gate of the second token
       const float u = odd ? mine1 : got;     // gate lane: partner's up of the first token
       const int m = mr + 8 * ((i >> 1) & 1), n = nc + 8 * (i >> 2) + (odd ? 1 : 0);
-      if (n < n_valid && m < args.M) {
-        const float act = bf16_round(g / (1.0f + expf(-g)));
-        out[(size_t)n * args.ld + (m >> 1)] = __float2bfloat16_rn(act * u);
-      }
+      if (n < n_valid && m < args.M) out[(size_t)n * args.ld + (m >> 1)] = __ushort_as_bfloat16(swiglu_bf16_bits(g, u));
     }
   }
 }
 
 // ---------------------------------------------------------------------------------
-// persistent-kernel epilogue through shared memory (bf16 and SwiGLU outputs): each consumer warpgroup writes
-// its 64 output features x BN tokens into its own 16 KiB staging buffer, then stores 16-byte pieces of output
-// rows.  Every value and rounding is the one gemm_store computes; only the way it reaches global memory
-// differs (from registers each warp store touches 4-8 rows with 2 bytes per lane).  Staging rows are 16-byte
-// chunks XOR-swizzled by the row index so that both the writes and the row reads are free of bank conflicts.
-// `tid` = thread in the warpgroup (0..127), `w4` = warp in the warpgroup.
+// persistent-kernel epilogue through shared memory (bf16 and SwiGLU outputs), split in two halves:
+//   gemm_stage_tile     consumer warpgroup `wg`: its 64 features x BN tokens of the finished tile, bf16-rounded
+//                       (the GEMM's own rounding point: pack_bf16x2), into its half of the staging buffer
+//   gemm_epilogue_tile  the epilogue warps: read the tile back, apply SwiGLU, store 16-byte pieces of output rows
+// Every value and rounding is the one gemm_store computes; only the way it reaches global memory differs (from
+// registers each warp store touches 4-8 rows with 2 bytes per lane).  A half is [token][64 features] rows of
+// 128 B whose 16-byte chunk c sits at chunk c ^ (row & 7), so that the stmatrix writes and the 16-byte row reads
+// are free of bank conflicts.  W rows are interleaved (gate_j, up_j), so for SwiGLU each staged gate value sits
+// next to its up value.
 // ---------------------------------------------------------------------------------
-// one staged piece of 8 outputs, columns [col, col + 8) of an output row: one 16-byte store, or element by
-// element where the piece runs past the last column (ragged M) or rows are not 16-byte aligned (!vec_ok)
-__device__ __forceinline__ void gemm_store_piece(__nv_bfloat16* row, int col, int ncols, bool vec_ok, uint32_t src) {
-  const uint4 v = lds_v4(src);
+// one piece of 8 outputs, columns [col, col + 8) of an output row: one 16-byte store, or element by element
+// where the piece runs past the last column (ragged M) or rows are not 16-byte aligned (!vec_ok)
+__device__ __forceinline__ void gemm_store_piece(__nv_bfloat16* row, int col, int ncols, bool vec_ok, uint4 v) {
   if (vec_ok && col + 8 <= ncols) {
     *(uint4*)(row + col) = v;
   } else {
@@ -295,64 +311,51 @@ __device__ __forceinline__ void gemm_store_piece(__nv_bfloat16* row, int col, in
       if (col + q < ncols) row[col + q] = __ushort_as_bfloat16((unsigned short)(w[q >> 1] >> (16 * (q & 1))));
   }
 }
-// bf16: rows of 64 features (128 B) per token, 128 tokens per pass (stmatrix .trans turns the [m][n]
+// `st` = the warpgroup's half of the buffer, `w4` = warp in the warpgroup (stmatrix .trans turns the [m][n]
 // accumulator fragments into [n][m] rows)
 template <int BN>
-__device__ __forceinline__ void gemm_store_staged_bf16(const float (&d)[BN / 2], const GemmArgs& args, uint8_t* stage, int m_wg0,
-                                                       int n0, int n_valid, bool vec_ok, int wg, int w4, int lane, int tid) {
-  constexpr int PASS_N = PGEMM_STAGE_BYTES / 128;
-  const uint32_t st = smem_u32(stage);
-  __nv_bfloat16* out = (__nv_bfloat16*)args.out;
+__device__ __forceinline__ void gemm_stage_tile(const float (&d)[BN / 2], uint32_t st, int w4, int lane) {
 #pragma unroll
-  for (int p = 0; p < BN / PASS_N + (BN < PASS_N ? 1 : 0); ++p) {
-    named_bar_sync(2 + wg, 128);   // the previous pass (or tile) has read the buffer
-#pragma unroll
-    for (int j = p * PASS_N / 8; j < (p + 1) * PASS_N / 8 && j < BN / 8; j += 2) {
-      // matrices (features 8h.., tokens 8j'..) for h = i & 1, j' = j + (i >> 1); this lane addresses token row k
-      const int i = lane >> 3, k = lane & 7;
-      const int n = 8 * (j - p * PASS_N / 8 + (i >> 1)) + k, c = 2 * w4 + (i & 1);
-      stmatrix_x4_trans(st + n * 128 + ((c ^ (n & 7)) << 4), pack_bf16x2(d[4 * j], d[4 * j + 1]),
-                        pack_bf16x2(d[4 * j + 2], d[4 * j + 3]), pack_bf16x2(d[4 * j + 4], d[4 * j + 5]),
-                        pack_bf16x2(d[4 * j + 6], d[4 * j + 7]));
-    }
-    named_bar_sync(2 + wg, 128);
-    constexpr int ROWS = BN < PASS_N ? BN : PASS_N;
-#pragma unroll
-    for (int it = 0; it < ROWS * 8 / 128; ++it) {
-      const int idx = it * 128 + tid, n = idx >> 3, c = idx & 7, gn = n0 + p * PASS_N + n;
-      if (gn < n_valid)
-        gemm_store_piece(out + (size_t)gn * args.ld, m_wg0 + 8 * c, args.M, vec_ok, st + n * 128 + ((c ^ (n & 7)) << 4));
-    }
+  for (int j = 0; j < BN / 8; j += 2) {
+    // matrices (features 8h.., tokens 8j'..) for h = i & 1, j' = j + (i >> 1); this lane addresses token row k
+    const int i = lane >> 3, k = lane & 7;
+    const int n = 8 * (j + (i >> 1)) + k, c = 2 * w4 + (i & 1);
+    stmatrix_x4_trans(st + n * 128 + ((c ^ (n & 7)) << 4), pack_bf16x2(d[4 * j], d[4 * j + 1]),
+                      pack_bf16x2(d[4 * j + 2], d[4 * j + 3]), pack_bf16x2(d[4 * j + 4], d[4 * j + 5]),
+                      pack_bf16x2(d[4 * j + 6], d[4 * j + 7]));
   }
 }
-
-// SwiGLU: rows of 32 outputs (64 B) per token, the whole tile in one pass; the arithmetic is gemm_store's
-template <int BN>
-__device__ __forceinline__ void gemm_store_staged_swiglu(const float (&d)[BN / 2], const GemmArgs& args, uint8_t* stage, int m_wg0,
-                                                         int n0, int n_valid, bool vec_ok, int wg, int w4, int lane, int tid) {
-  static_assert(BN * 64 <= PGEMM_STAGE_BYTES, "one pass");
-  const uint32_t st = smem_u32(stage);
-  const bool odd = (lane >> 2) & 1;
-  named_bar_sync(2 + wg, 128);
-#pragma unroll
-  for (int i = 0; i < BN / 2; i += 2) {
-    const float mine0 = bf16_round(d[i]);
-    const float mine1 = bf16_round(d[i + 1]);
-    const float got = __shfl_xor_sync(0xffffffffu, odd ? mine0 : mine1, 4);
-    const float g = odd ? got : mine0;
-    const float u = odd ? mine1 : got;
-    const float act = bf16_round(g / (1.0f + expf(-g)));
-    const int col = (16 * w4 + (lane >> 2) + 8 * ((i >> 1) & 1)) >> 1;          // output column in the warpgroup
-    const int n = 2 * (lane & 3) + 8 * (i >> 2) + (odd ? 1 : 0);                 // token in the tile
-    sts_u16(st + n * 64 + (((col >> 3) ^ ((n >> 1) & 3)) << 4) + (col & 7) * 2, f32_to_bf16_bits(act * u));
-  }
-  named_bar_sync(2 + wg, 128);
+// Tile (features m0 .. m0 + 127, tokens n0 .. n0 + BN - 1) from the buffer at `st`; `et` = epilogue thread (0..95).
+// bf16: a token row is 16 pieces (8 per half).  SwiGLU: a piece of 8 outputs is two adjacent staged chunks of
+// 4 (gate, up) pairs; threads 4r.. take rows 2r, 2r + 1 so that a phase of 8 lanes reads distinct banks.
+template <int BN, int EPI>
+__device__ __forceinline__ void gemm_epilogue_tile(const GemmArgs& args, uint32_t st, int m0, int n0, int n_valid, bool vec_ok,
+                                                   int et) {
+  constexpr uint32_t HALF = BN * 128;
+  const int rows = min(BN, n_valid - n0);
   __nv_bfloat16* out = (__nv_bfloat16*)args.out;
+  if constexpr (EPI == EPI_BF16) {
+    for (int idx = et; idx < rows * 16; idx += PGEMM_EPI_THREADS) {
+      const int n = idx >> 4, h = (idx >> 3) & 1, c = idx & 7;
+      gemm_store_piece(out + (size_t)(n0 + n) * args.ld, m0 + 64 * h + 8 * c, args.M, vec_ok,
+                       lds_v4(st + h * HALF + n * 128 + ((c ^ (n & 7)) << 4)));
+    }
+  } else {
+    static_assert(EPI == EPI_SWIGLU, "bf16 or SwiGLU");
+    for (int idx = et; idx < ((rows + 1) & ~1) * 8; idx += PGEMM_EPI_THREADS) {
+      const int c = idx & 3, h = (idx >> 3) & 1, n = 2 * (idx >> 4) + ((idx >> 2) & 1);
+      if (n >= rows) continue;
+      const uint32_t row = st + h * HALF + n * 128;
+      const uint4 a = lds_v4(row + (((2 * c) ^ (n & 7)) << 4)), b = lds_v4(row + (((2 * c + 1) ^ (n & 7)) << 4));
+      const uint32_t gu[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};   // output 8c + q: gate low, up high half
+      uint32_t o[4];
 #pragma unroll
-  for (int it = 0; it < BN * 4 / 128; ++it) {
-    const int idx = it * 128 + tid, n = idx >> 2, c = idx & 3, gn = n0 + n;
-    if (gn < n_valid)
-      gemm_store_piece(out + (size_t)gn * args.ld, (m_wg0 >> 1) + 8 * c, args.M >> 1, vec_ok, st + n * 64 + ((c ^ ((n >> 1) & 3)) << 4));
+      for (int q = 0; q < 4; ++q)
+        o[q] = (uint32_t)swiglu_bf16_bits(bf16_lo(gu[2 * q]), bf16_hi(gu[2 * q])) |
+               ((uint32_t)swiglu_bf16_bits(bf16_lo(gu[2 * q + 1]), bf16_hi(gu[2 * q + 1])) << 16);
+      gemm_store_piece(out + (size_t)(n0 + n) * args.ld, ((m0 + 64 * h) >> 1) + 8 * c, args.M >> 1, vec_ok,
+                       make_uint4(o[0], o[1], o[2], o[3]));
+    }
   }
 }
 
@@ -511,20 +514,28 @@ gemm_wx_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant
 // Both CTAs walk the same pairs in lockstep, so their rings advance stage for stage: each loads its own W
 // tile and multicasts half of the X tile to both (`tmap_xh`: a box of BN/2 token rows; gemm_produce_pair).
 // bf16, SwiGLU or one fp32 plane.
+// Roles: thread 0 is the producer; warps 1-3 (bf16 and SwiGLU) are the epilogue role, which stores tile t from the
+// staging buffer while the consumer warpgroups (warps 4-11) run tile t + 1's MMAs.  Two mbarriers hand the buffer
+// back and forth: `staged` (256 consumer threads arrive once the tile is written) and `released` (96 epilogue
+// threads arrive once it is read).  The fp32 plane is stored by the consumers from registers.
 template <int EPI, bool FP8 = false>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_xh,
                           GemmArgs args, int m_tiles, int n_tiles) {
   constexpr int BN = FP8 ? PGEMM_BN_E4M3 : PGEMM_BN;
   using Cfg = GemmCfg<BN>;
-  constexpr int STAGES = Cfg::kStages;
+  constexpr int STAGES = PGemmStages<EPI, FP8>;
   constexpr int BK = FP8 ? GEMM_BK_E4M3 : GEMM_BK;
+  constexpr bool STAGED = EPI != EPI_F32;
   extern __shared__ uint8_t smem_raw[];
   // the same alignment in both CTAs of the cluster (the dynamic shared window starts at the same offset), so
   // a multicast box lands at the same offset of the ring in each
   uint8_t* smem = (uint8_t*)(((uintptr_t)smem_raw + 1023) & ~(uintptr_t)1023);
   uint64_t* full_bar = (uint64_t*)(smem + STAGES * Cfg::kStageBytes);
   uint64_t* empty_bar = full_bar + STAGES;
+  uint64_t* staged_bar = empty_bar + STAGES;
+  uint64_t* released_bar = staged_bar + 1;
+  const uint32_t staging = smem_u32(smem + STAGES * Cfg::kStageBytes + 256);   // PGemmSmem: past the barriers
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -532,12 +543,16 @@ gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __gr
   const int cluster = (int)blockIdx.x >> 1, clusters = (int)gridDim.x >> 1;
   const int nkb = (args.K + BK - 1) / BK;
   const int num_pairs = ((m_tiles + 1) >> 1) * n_tiles;
+  // 16-byte stores need output rows that start 16-byte aligned
+  const bool vec_ok = args.ld % 8 == 0 && ((uintptr_t)args.out & 15) == 0;
 
   pdl_launch_dependents();
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_xh);
     for (int s = 0; s < STAGES; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 16); }
+    mbar_init(staged_bar, 256);
+    mbar_init(released_bar, PGEMM_EPI_THREADS);
     fence_mbar_init();
   }
   cluster_sync_relaxed();   // both CTAs' barriers are initialised before either multicasts or arrives on them
@@ -552,14 +567,27 @@ gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __gr
         gemm_produce_pair<BN, STAGES, BK>(smem, full_bar, empty_bar, s, ph, &tmap_w, &tmap_xh, m_tile * nkb * GEMM_BM,
                                           m_tile < m_tiles, nkb, (p % n_tiles) * BN, rank);
       }
+    } else if constexpr (STAGED) {
+      if (warp > 0) {
+        // ===== epilogue role: the tiles with a W tile, in the consumers' order =====
+        pdl_wait();   // the previous kernel may still read the output buffer
+        const int n_valid = args.n_dev ? *args.n_dev : args.N;
+        uint32_t eph = 0;
+        for (int p = cluster; p < num_pairs; p += clusters) {
+          const int m_tile = 2 * (p / n_tiles) + (int)rank;
+          if (m_tile >= m_tiles) continue;
+          mbar_wait_mma(staged_bar, eph);
+          gemm_epilogue_tile<BN, EPI>(args, staging, m_tile * GEMM_BM, (p % n_tiles) * BN, n_valid, vec_ok, threadIdx.x - 32);
+          mbar_arrive(released_bar);
+          eph ^= 1;
+        }
+      }
     }
   } else {
-    const int wg = (warp >> 2) - 1, cw = warp - 4, tid = threadIdx.x & 127;
-    uint8_t* stage = (uint8_t*)(empty_bar + STAGES) + wg * PGEMM_STAGE_BYTES;   // PGemmSmem: past the barriers
-    // 16-byte stores need output rows that start 16-byte aligned
-    const bool vec_ok = args.ld % 8 == 0 && ((uintptr_t)args.out & 15) == 0;
+    const int wg = (warp >> 2) - 1, cw = warp - 4;
     pdl_wait();
     const int n_valid = args.n_dev ? *args.n_dev : args.N;
+    uint32_t eph = 0;   // parity of the staging-buffer hand-over
     for (int p = cluster; p < num_pairs; p += clusters) {
       const int m_tile = 2 * (p / n_tiles) + (int)rank, m_base = m_tile * GEMM_BM + cw * 16, n0 = (p % n_tiles) * BN;
       float d[BN / 2];
@@ -568,10 +596,14 @@ gemm_wx_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __gr
       else gemm_consume<BN, STAGES, true>(d, smem, full_bar, empty_bar, s, ph, nkb, wg, lane, rank);
       if (m_tile < m_tiles) {
         if constexpr (FP8) gemm_scale_e4m3<BN>(d, args, m_base, n0, 0, n_valid, lane);
-        const int m_wg0 = m_tile * GEMM_BM + 64 * wg;
-        if constexpr (EPI == EPI_BF16) gemm_store_staged_bf16<BN>(d, args, stage, m_wg0, n0, n_valid, vec_ok, wg, cw & 3, lane, tid);
-        else if constexpr (EPI == EPI_SWIGLU) gemm_store_staged_swiglu<BN>(d, args, stage, m_wg0, n0, n_valid, vec_ok, wg, cw & 3, lane, tid);
-        else gemm_store<BN, EPI>(d, args, m_base, n0, 0, n_valid, 0, lane);   // the fp32 plane, from registers
+        if constexpr (STAGED) {
+          mbar_wait_mma(released_bar, eph ^ 1);   // the epilogue warps have read the previous tile
+          gemm_stage_tile<BN>(d, staging + wg * (BN * 128), cw & 3, lane);
+          mbar_arrive(staged_bar);
+          eph ^= 1;
+        } else {
+          gemm_store<BN, EPI>(d, args, m_base, n0, 0, n_valid, 0, lane);   // the fp32 plane, from registers
+        }
       }
     }
   }

@@ -17,6 +17,19 @@ struct DevBuf {
   ~DevBuf() { if (p) cudaFree(p); }
   int alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 1) == cudaSuccess ? 0 : -5; }
 };
+// Every GEMM output buffer is followed by kGuardBytes of 0xff: a store past the end of the output ([N][ld], or
+// the split-K planes) changes one, and the hook returns ACP_ERR_GUARD instead of the result.
+constexpr size_t kGuardBytes = 4096;
+int check_guard(const DevBuf& out, size_t out_bytes) {
+  std::vector<uint8_t> g(kGuardBytes);
+  if (cudaMemcpy(g.data(), (const uint8_t*)out.p + out_bytes, kGuardBytes, cudaMemcpyDeviceToHost) != cudaSuccess) return -5;
+  for (uint8_t b : g)
+    if (b != 0xff) {
+      fprintf(stderr, "[acp_infer] GEMM store past the end of the output buffer (%zu bytes)\n", out_bytes);
+      return ACP_ERR_GUARD;
+    }
+  return 0;
+}
 __global__ void l2_flush_kernel(float* buf, size_t n) {
   size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
   size_t stride = (size_t)gridDim.x * blockDim.x;
@@ -72,8 +85,8 @@ extern "C" int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int 
   else if (epi == EPI_F32) out_bytes = (size_t)splits * N * M * 4;
   else if (epi == EPI_SWIGLU) out_bytes = (size_t)N * (M / 2) * 2;
   else if (out != nullptr) out_bytes = (size_t)N * M * 4;
-  if (dout.alloc(out_bytes)) return -5;
-  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes ? out_bytes : 1));
+  if (dout.alloc(out_bytes + kGuardBytes)) return -5;
+  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes + kGuardBytes));
   if (epi == EPI_ARGMAX) {
     if (dval.alloc((size_t)N * m_tiles * 4) || didx.alloc((size_t)N * m_tiles * 4)) return -5;
   }
@@ -88,6 +101,7 @@ extern "C" int acp_kernel_gemm(const uint16_t* w, const uint16_t* x, int M, int 
   int rc = gemm_launch(g, 0);
   if (rc != 0) return rc;
   ACP_CUDA_CHECK(cudaDeviceSynchronize());
+  if ((rc = check_guard(dout, out_bytes)) != 0) return rc;
   if (out != nullptr && out_bytes)
     ACP_CUDA_CHECK(cudaMemcpy(out, dout.p, out_bytes, cudaMemcpyDeviceToHost));
   if (epi == EPI_ARGMAX) {
@@ -306,8 +320,8 @@ extern "C" int acp_kernel_gemm_fp8(const uint8_t* w, const float* w_scale, const
   else if (epi == EPI_F32) out_bytes = (size_t)splits * N * M * 4;
   else if (epi == EPI_SWIGLU) out_bytes = (size_t)N * (M / 2) * 2;
   else return -1;
-  if (dout.alloc(out_bytes)) return -5;
-  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes));
+  if (dout.alloc(out_bytes + kGuardBytes)) return -5;
+  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes + kGuardBytes));
   TmaMaps mw, mx;
   if (tma_make_weight_e4m3(&mw, dw.p, Mp, Kp) != 0) return -5;
   if (tma_make_act_e4m3(&mx, dx.p, n_pad, Kp) != 0) return -5;
@@ -318,6 +332,7 @@ extern "C" int acp_kernel_gemm_fp8(const uint8_t* w, const float* w_scale, const
   int rc = gemm_launch(g, 0);
   if (rc != 0) return rc;
   ACP_CUDA_CHECK(cudaDeviceSynchronize());
+  if ((rc = check_guard(dout, out_bytes)) != 0) return rc;
   ACP_CUDA_CHECK(cudaMemcpy(out, dout.p, out_bytes, cudaMemcpyDeviceToHost));
   if (iters > 0 && elapsed_ms != nullptr) return time_launches([&] { return gemm_launch(g, 0); }, iters, elapsed_ms);
   return 0;

@@ -11,6 +11,9 @@
 #define ACP_INFER_KERNELS_H
 #include <stddef.h>
 #include <stdint.h>
+/* acp_kernel_gemm / acp_kernel_gemm_fp8: a kernel stored past the end of the output */
+#define ACP_ERR_GUARD (-8)
+
 #ifdef __cplusplus
 extern "C" {
 #endif
@@ -21,6 +24,7 @@ extern "C" {
  * fp32 logits [N][M] (may be NULL); epi 3: rows of w interleaved (gate_j, up_j), out = bf16
  * [N][M/2] = bf16(bf16(silu(g)) * u).  bn = 0 picks the N tile from N; otherwise 16..256;
  * bn = -1 (N > 256, epi 0, 1 or 3) forces the persistent prefill kernel.
+ * The output buffer is followed by a guard region; a store past its end returns ACP_ERR_GUARD.
  * iters > 0 additionally times `iters` launches with CUDA events (L2 flushed between
  * launches) and stores the mean milliseconds in *elapsed_ms; iters < 0 is a stress mode: -iters launches back
  * to back (no flush, one synchronize at the end), mean milliseconds in *elapsed_ms. */

@@ -1,6 +1,7 @@
 """BASELINE config 2: Llama-3-8B, 256 concurrent Tasks, prompt lengths log-uniform on [128, 4096]
 (seeded), continuous batching, max_tokens 64, 1 GPU.  Prints engine stats as JSON.
-usage: python scripts/config2_probe.py [n_tasks] [max_tokens] [layers]"""
+usage: python scripts/config2_probe.py [n_tasks] [max_tokens] [layers]
+MAX_TOKENS_PER_STEP (default 8192) sets the engine's token rows per prefill step; bench.py runs 4096."""
 import json
 import os
 import sys
@@ -16,7 +17,7 @@ max_new = int(sys.argv[2]) if len(sys.argv) > 2 else 64
 rng = np.random.default_rng(0xC0F162)
 lens = np.exp(rng.uniform(np.log(128), np.log(4096), size=n)).astype(int)
 pages = int(sum((l + max_new) // 32 + 2 for l in lens)) + 64
-cfg = {"model": "llama-3-8b", "max_batch": n, "kv_pages": pages, "max_tokens_per_step": 8192,
+cfg = {"model": "llama-3-8b", "max_batch": n, "kv_pages": pages, "max_tokens_per_step": int(os.environ.get("MAX_TOKENS_PER_STEP", "8192")),
        "max_pages_per_seq": (4096 + max_new) // 32 + 2, "prefix_cache": False}
 if len(sys.argv) > 3:
     cfg["layers"] = int(sys.argv[3])
