@@ -13,6 +13,7 @@
 #include "gemm_wgmma.cuh"
 #include "fp8.h"
 #include <math.h>
+#include <algorithm>
 #include <stdlib.h>
 #include <string.h>
 
@@ -187,14 +188,8 @@ int Model::init(const ModelConfig& cfg, const ModelLimits& lim, int device, int 
   }
   const char* env = getenv("ACP_SPLITK_TARGET");
   if (env) lim_.splitk_target_ctas = atoi(env);
-  env = getenv("ACP_FUSE_SWIGLU");
-  fuse_swiglu_ = env && *env == '1';
-  // Prefill: SwiGLU runs in the persistent gate/up GEMM's epilogue (paired-lane exchange; the producer
-  // streams the next tile meanwhile).  ACP_FUSE_SWIGLU_PREFILL=0 restores the separate kernel.
   env = getenv("ACP_TP_SYNC_EVERY");
   tp_sync_every_ = (env && tp_size > 1) ? atoi(env) : 0;
-  env = getenv("ACP_FUSE_SWIGLU_PREFILL");
-  fuse_swiglu_prefill_ = !(env && *env == '0');
   ACP_CUDA_CHECK(cudaSetDevice(device));
   ACP_CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   ACP_TRY(tma_init());
@@ -208,56 +203,83 @@ int Model::init(const ModelConfig& cfg, const ModelLimits& lim, int device, int 
   return 0;
 }
 
+// Where this shard's weights sit in the logical tensors that oracle/synth.py generates and a checkpoint
+// stores: the only place the projection, LM head and expert layouts are written.  The generator and the
+// loader both place weights through these maps.
+void Model::describe_weights() {
+  const ModelConfig& c = cfg_;
+  const int H = c.hidden, r = tp_rank_;
+  // gate/up rows interleaved (2j = gate_j, 2j+1 = up_j), from row `row0` of each half of the logical [gate; up]
+  auto gate_up = [&](int half, int row0) {
+    SynthMap m{H, H, 0, half};
+    m.seg_global[0] = row0;
+    m.seg_global[1] = c.ffn + row0;
+    return m;
+  };
+  SynthMap qkv{H, H, 0};   // [q heads of this rank | k heads | v heads] rows of the logical [q; k; v]
+  qkv.nseg = 3;
+  qkv.seg_rows[0] = qdim_l_; qkv.seg_global[0] = r * qdim_l_;
+  qkv.seg_rows[1] = kvdim_l_; qkv.seg_global[1] = c.q_dim() + r * kvdim_l_;
+  qkv.seg_rows[2] = kvdim_l_; qkv.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
+  for (Layer& L : layers_) {
+    L.qkv = Proj{qkv_l_, H, qkv, 0, {{"self_attn.q_proj", c.q_dim()}, {"self_attn.k_proj", c.kv_dim()}, {"self_attn.v_proj", c.kv_dim()}}};
+    L.o = Proj{H, qdim_l_, SynthMap{qdim_l_, c.q_dim(), r * qdim_l_}, 1, {{"self_attn.o_proj", H}}};
+    if (c.experts > 0) continue;
+    L.gu = Proj{2 * ffn_l_, H, gate_up(ffn_l_, r * ffn_l_), 2, {{"mlp.gate_proj", c.ffn}, {"mlp.up_proj", c.ffn}}};
+    L.down = Proj{H, ffn_l_, SynthMap{ffn_l_, c.ffn, r * ffn_l_}, 3, {{"mlp.down_proj", H}}};
+  }
+  lm_map_ = SynthMap{H, H, 0};   // this shard's rows, contiguous in the logical tensor
+  lm_map_.nseg = 1; lm_map_.seg_rows[0] = lm_rows_l_; lm_map_.seg_global[0] = lm_row0_;
+  gu_e_map_ = gate_up(c.ffn, 0);   // whole experts
+  down_e_map_ = SynthMap{c.ffn, c.ffn, 0};
+}
+
+// Allocates and maps p: bf16 tiles, or e4m3 tiles and row scales under cfg.fp8.  Grows the split-K workspace
+// to what p's decode GEMMs need at any step height (the split factor depends on it beyond 256 rows, model_config.cc).
+int Model::alloc_proj(Proj& p) {
+  const ModelLimits& m = lim_;
+  if (cfg_.fp8) {
+    ws_bytes_ = std::max(ws_bytes_, splitk_workspace_bytes_fp8(p.M, p.K, m.max_batch, m.splitk_target_ctas, m.strict_batch_invariance));
+    ACP_TRY(dmalloc_t(allocs_, &p.codes, (size_t)p.M * p.K));
+    ACP_TRY(dmalloc_t(allocs_, &p.scale, (size_t)p.M));
+    return tma_make_weight_e4m3(&p.m, p.codes, p.M, p.K);
+  }
+  ws_bytes_ = std::max(ws_bytes_, splitk_workspace_bytes(p.M, p.K, m.max_batch, m.splitk_target_ctas, m.strict_batch_invariance));
+  ACP_TRY(dmalloc_t(allocs_, &p.w, (size_t)p.M * p.K));
+  return tma_make_weight(&p.m, p.w, p.M, p.K);
+}
+
+// Allocates (zeroed) an activation, and under cfg.fp8 its e4m3 copy and row scales; maps the one GEMMs read
+int Model::alloc_act(Act& a, int rows, int cols, const char* quant) {
+  a.quant = quant;
+  ACP_TRY(dmalloc_t(allocs_, &a.x, (size_t)rows * cols, true));
+  if (!cfg_.fp8) return tma_make_act(&a.m, a.x, rows, cols);
+  ACP_TRY(dmalloc_t(allocs_, &a.x8, (size_t)rows * cols, true));
+  ACP_TRY(dmalloc_t(allocs_, &a.scale, (size_t)rows, true));
+  return tma_make_act_e4m3(&a.m, a.x8, rows, cols);
+}
+
 int Model::alloc_all() {
   const ModelConfig& c = cfg_;
   const size_t H = c.hidden;
   const int T = ((lim_.max_tokens + 255) / 256) * 256;
   const int Bp = ((lim_.max_batch + 255) / 256) * 256;
   layers_.resize(c.layers);
+  describe_weights();
   const size_t kv_elems = (size_t)lim_.num_pages * kvh_l_ * KV_PAGE * HEAD_DIM;
-  for (int l = 0; l < c.layers; ++l) {
-    Layer& L = layers_[l];
-    if (c.fp8) {
-      ACP_TRY(dmalloc_t(allocs_, &L.wqkv8, (size_t)qkv_l_ * H));
-      ACP_TRY(dmalloc_t(allocs_, &L.wo8, H * qdim_l_));
-      ACP_TRY(dmalloc_t(allocs_, &L.wgu8, (size_t)2 * ffn_l_ * H));
-      ACP_TRY(dmalloc_t(allocs_, &L.wdown8, H * ffn_l_));
-      ACP_TRY(dmalloc_t(allocs_, &L.s_qkv, (size_t)qkv_l_));
-      ACP_TRY(dmalloc_t(allocs_, &L.s_o, H));
-      ACP_TRY(dmalloc_t(allocs_, &L.s_gu, (size_t)2 * ffn_l_));
-      ACP_TRY(dmalloc_t(allocs_, &L.s_down, H));
-      ACP_TRY(tma_make_weight_e4m3(&L.m_qkv, L.wqkv8, qkv_l_, H));
-      ACP_TRY(tma_make_weight_e4m3(&L.m_o, L.wo8, H, qdim_l_));
-      ACP_TRY(tma_make_weight_e4m3(&L.m_gu, L.wgu8, 2 * ffn_l_, H));
-      ACP_TRY(tma_make_weight_e4m3(&L.m_down, L.wdown8, H, ffn_l_));
-      L.wqkv = L.wo = L.wgu = L.wdown = nullptr;
-    } else {
-      ACP_TRY(dmalloc_t(allocs_, &L.wqkv, (size_t)qkv_l_ * H));
-      ACP_TRY(dmalloc_t(allocs_, &L.wo, H * qdim_l_));
-    }
+  for (Layer& L : layers_) {
+    for (Proj* p : L.projs()) ACP_TRY(alloc_proj(*p));
     if (c.experts > 0) {
       ACP_TRY(dmalloc_t(allocs_, &L.router, (size_t)c.experts * H));
       ACP_TRY(dmalloc_t(allocs_, &L.wgu_e, (size_t)experts_l_ * 2 * c.ffn * H));
       ACP_TRY(dmalloc_t(allocs_, &L.wdown_e, (size_t)experts_l_ * H * c.ffn));
       ACP_TRY(tma_make_weight(&L.m_gu_e, L.wgu_e, (uint64_t)experts_l_ * 2 * c.ffn, H));
       ACP_TRY(tma_make_weight(&L.m_down_e, L.wdown_e, (uint64_t)experts_l_ * H, c.ffn));
-      L.wgu = L.wdown = nullptr;
-    } else if (!c.fp8) {
-      ACP_TRY(dmalloc_t(allocs_, &L.wgu, (size_t)2 * ffn_l_ * H));
-      ACP_TRY(dmalloc_t(allocs_, &L.wdown, H * ffn_l_));
     }
     ACP_TRY(dmalloc_t(allocs_, &L.attn_norm, H));
     ACP_TRY(dmalloc_t(allocs_, &L.ffn_norm, H));
     ACP_TRY(dmalloc_t(allocs_, &L.k_cache, kv_elems, true));
     ACP_TRY(dmalloc_t(allocs_, &L.v_cache, kv_elems, true));
-    if (!c.fp8) {
-      ACP_TRY(tma_make_weight(&L.m_qkv, L.wqkv, qkv_l_, H));
-      ACP_TRY(tma_make_weight(&L.m_o, L.wo, H, qdim_l_));
-    }
-    if (c.experts == 0 && !c.fp8) {
-      ACP_TRY(tma_make_weight(&L.m_gu, L.wgu, 2 * ffn_l_, H));
-      ACP_TRY(tma_make_weight(&L.m_down, L.wdown, H, ffn_l_));
-    }
     ACP_TRY(attn_make_kv_map(&L.tm_k, L.k_cache, lim_.num_pages, kvh_l_));
     ACP_TRY(attn_make_kv_map(&L.tm_v, L.v_cache, lim_.num_pages, kvh_l_));
     ACP_TRY(attn_make_kv_half_map(&L.tm_k32, L.k_cache, lim_.num_pages, kvh_l_));
@@ -271,10 +293,10 @@ int Model::alloc_all() {
   ACP_TRY(dmalloc_t(allocs_, &sin_, (size_t)c.max_pos * 64));
   // activations (rows padded to the largest N tile, zero initialised)
   ACP_TRY(dmalloc_t(allocs_, &x_, (size_t)T * H, true));
-  ACP_TRY(dmalloc_t(allocs_, &xn_, (size_t)T * H, true));
+  ACP_TRY(alloc_act(xn_, T, c.hidden, "quant_xn"));
   ACP_TRY(dmalloc_t(allocs_, &qbuf_, (size_t)T * qdim_l_, true));
-  ACP_TRY(dmalloc_t(allocs_, &attn_, (size_t)T * qdim_l_, true));
-  ACP_TRY(dmalloc_t(allocs_, &h_, (size_t)T * (c.experts > 0 ? 8 : ffn_l_), true));
+  ACP_TRY(alloc_act(attn_, T, qdim_l_, "quant_attn"));
+  if (c.experts == 0) ACP_TRY(alloc_act(h_, T, ffn_l_, "quant_h"));
   if (c.experts > 0) {
     const size_t rows = (size_t)2 * T + 256;   // 2 assignments per token, + one N tile of slack for the last group's TMA box
     ACP_TRY(dmalloc_t(allocs_, &xe_, rows * H, true));
@@ -288,46 +310,20 @@ int Model::alloc_all() {
     ACP_TRY(dmalloc_t(allocs_, &moe_ranges_, (size_t)moe_ranges_ints(T), true));
   }
   ACP_TRY(dmalloc_t(allocs_, &xs_, (size_t)Bp * H, true));
-  int max_m = qkv_l_;
-  if (2 * ffn_l_ > max_m) max_m = 2 * ffn_l_;
-  if (c.hidden > max_m) max_m = c.hidden;
+  size_t max_m = H;   // gemm_bf16_: the output of one dense GEMM or of the expert combine
+  for (const Proj* p : layers_[0].projs()) max_m = std::max(max_m, (size_t)p->M);
   ACP_TRY(dmalloc_t(allocs_, &gemm_bf16_, (size_t)T * max_m, true));
   ACP_TRY(attn_make_q_map(&tm_q_, qbuf_, (uint64_t)T, heads_l_, kvh_l_));
-  ACP_TRY(tma_make_act(&m_xn_, xn_, T, H));
-  ACP_TRY(tma_make_act(&m_attn_, attn_, T, qdim_l_));
-  if (c.experts == 0) ACP_TRY(tma_make_act(&m_h_, h_, T, ffn_l_));
   ACP_TRY(tma_make_act(&m_xs_, xs_, Bp, H));
-  if (c.fp8) {
-    ACP_TRY(dmalloc_t(allocs_, &xn8_, (size_t)T * H, true));
-    ACP_TRY(dmalloc_t(allocs_, &attn8_, (size_t)T * qdim_l_, true));
-    ACP_TRY(dmalloc_t(allocs_, &h8_, (size_t)T * ffn_l_, true));
-    ACP_TRY(dmalloc_t(allocs_, &sx_xn_, (size_t)T, true));
-    ACP_TRY(dmalloc_t(allocs_, &sx_attn_, (size_t)T, true));
-    ACP_TRY(dmalloc_t(allocs_, &sx_h_, (size_t)T, true));
-    ACP_TRY(tma_make_act_e4m3(&m_xn8_, xn8_, T, H));
-    ACP_TRY(tma_make_act_e4m3(&m_attn8_, attn8_, T, qdim_l_));
-    ACP_TRY(tma_make_act_e4m3(&m_h8_, h8_, T, ffn_l_));
-  }
-  // split-K workspace: worst case over the four GEMMs of a decode step with max_batch rows
-  size_t ws = 0;
-  const int shapes[4][2] = {{qkv_l_, c.hidden}, {c.hidden, qdim_l_}, {2 * ffn_l_, c.hidden}, {c.hidden, ffn_l_}};
-  for (auto& s : shapes) {
-    if (c.experts > 0 && (&s - shapes) >= 2) continue;   // the expert GEMMs are grouped, never split-K
-    // the split factor depends on the row count beyond 256 rows: sized over every step height (model_config.cc)
-    const size_t b = c.fp8 ? splitk_workspace_bytes_fp8(s[0], s[1], lim_.max_batch, lim_.splitk_target_ctas, lim_.strict_batch_invariance)
-                           : splitk_workspace_bytes(s[0], s[1], lim_.max_batch, lim_.splitk_target_ctas, lim_.strict_batch_invariance);
-    if (b > ws) ws = b;
-  }
+  // split-K workspace: alloc_proj sized it for the dense decode GEMMs (the expert GEMMs are grouped, never split-K)
   if (tp_size_ > 1) {  // row-parallel GEMMs write fp32 (one rounding after the all-reduce), prefill too
-    const size_t b = (size_t)T * H * sizeof(float);
-    if (b > ws) ws = b;
+    ws_bytes_ = std::max(ws_bytes_, (size_t)T * H * sizeof(float));
     ACP_TRY(dmalloc_t(allocs_, &ar_buf_, (size_t)T * H));
     ACP_TRY(dmalloc_t(allocs_, &cand_local_, (size_t)2 * Bp));
     ACP_TRY(dmalloc_t(allocs_, &cand_all_, (size_t)2 * Bp * tp_size_));
     ACP_TRY(dmalloc_t(allocs_, &amax_val_row_, (size_t)Bp));
     ACP_TRY(dmalloc_t(allocs_, &tp_flags_, (size_t)TP_MAX + 8, true));  // [0..7] flags, [8] done counter
   }
-  ws_bytes_ = ws;
   ACP_TRY(dmalloc(allocs_, (void**)&ws_, ws_bytes_));
   const int m_tiles_lm = (lm_rows_l_ + GEMM_BM - 1) / GEMM_BM;
   ACP_TRY(dmalloc_t(allocs_, &amax_val_, (size_t)Bp * m_tiles_lm));
@@ -355,95 +351,46 @@ int Model::alloc_all() {
 int Model::gen_weights() {
   const ModelConfig& c = cfg_;
   const size_t H = c.hidden;
-  // tensor ids shared with oracle/synth.py; SynthMap places this shard inside the logical tensors
-  auto tiled = [&](int local_cols, int logical_cols, int col0) {
-    SynthMap m;
-    m.local_cols = local_cols; m.logical_cols = logical_cols; m.col0 = col0;
-    return m;
-  };
+  // tensor ids shared with oracle/synth.py
   ACP_TRY(launch_synth(embed_, (size_t)c.vocab * H, c.seed, 1, c.w_std, 0, stream_));  // replicated, row-major
-  {
-    SynthMap m = tiled((int)H, (int)H, 0);
-    m.nseg = 1; m.seg_rows[0] = lm_rows_l_; m.seg_global[0] = lm_row0_;
-    ACP_TRY(launch_synth(lm_head_, (size_t)lm_rows_l_ * H, c.seed, 2, c.w_std, 0, stream_, m));
-  }
+  ACP_TRY(launch_synth(lm_head_, (size_t)lm_rows_l_ * H, c.seed, 2, c.w_std, 0, stream_, lm_map_));
   ACP_TRY(launch_synth(final_norm_, H, c.seed, 3, 0.1, 1, stream_));
   // FP8 presets: each projection is generated in bf16 into one staging buffer, quantised row by row into its
-  // e4m3 tiles + scales, and the bf16 copy is freed at the end
+  // e4m3 tiles + scales, and the staging buffer is freed at the end
   __nv_bfloat16* stage = nullptr;
   if (c.fp8) {
-    size_t n = (size_t)qkv_l_ * H;
-    if ((size_t)2 * ffn_l_ * H > n) n = (size_t)2 * ffn_l_ * H;
-    if (H * qdim_l_ > n) n = H * qdim_l_;
+    size_t n = 0;
+    for (const Proj* p : layers_[0].projs()) n = std::max(n, (size_t)p->M * p->K);
     ACP_CUDA_CHECK(cudaMalloc((void**)&stage, n * sizeof(__nv_bfloat16)));
   }
-  int rc = 0;
-  for (int l = 0; l < c.layers && rc == 0; ++l)
-    rc = gen_layer_weights(l, stage);
-  if (stage) {
-    ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    cudaFree(stage);
-  }
-  return rc;
-}
-
-// Layer l's synthetic tensors.  `stage` (FP8 presets) receives each bf16 projection before it is quantised.
-int Model::gen_layer_weights(int l, __nv_bfloat16* stage) {
-  const ModelConfig& c = cfg_;
-  const size_t H = c.hidden;
-  const int r = tp_rank_;
-  auto tiled = [&](int local_cols, int logical_cols, int col0) {
-    SynthMap m;
-    m.local_cols = local_cols; m.logical_cols = logical_cols; m.col0 = col0;
-    return m;
-  };
-  Layer& L = layers_[l];
-  {
+  auto gen_layer = [&](int l) -> int {
+    Layer& L = layers_[l];
     const uint32_t base = 16 + (uint32_t)l * 16;
-    auto dst = [&](__nv_bfloat16* w) { return stage ? stage : w; };
-    // FP8: quantise the projection just generated in `stage` (a tiled bf16 [M][K] matrix)
-    auto quant = [&](uint8_t* codes, float* scales, int M, int K) {
-      return stage ? launch_quantize_weight_e4m3(stage, M, K, codes, scales, stream_) : 0;
-    };
-    {  // [q heads of this rank | k heads | v heads] rows of the logical [q | k | v] tensor
-      SynthMap m = tiled((int)H, (int)H, 0);
-      m.nseg = 3;
-      m.seg_rows[0] = qdim_l_; m.seg_global[0] = r * qdim_l_;
-      m.seg_rows[1] = kvdim_l_; m.seg_global[1] = c.q_dim() + r * kvdim_l_;
-      m.seg_rows[2] = kvdim_l_; m.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
-      ACP_TRY(launch_synth(dst(L.wqkv), (size_t)qkv_l_ * H, c.seed, base + 0, c.w_std, 0, stream_, m));
-      ACP_TRY(quant(L.wqkv8, L.s_qkv, qkv_l_, (int)H));
+    for (const Proj* p : L.projs()) {
+      ACP_TRY(launch_synth(c.fp8 ? stage : p->w, (size_t)p->M * p->K, c.seed, base + p->tid, c.w_std, 0, stream_, p->map));
+      if (c.fp8) ACP_TRY(launch_quantize_weight_e4m3(stage, p->M, p->K, p->codes, p->scale, stream_));
     }
-    ACP_TRY(launch_synth(dst(L.wo), H * qdim_l_, c.seed, base + 1, c.w_std, 0, stream_, tiled(qdim_l_, c.q_dim(), r * qdim_l_)));
-    ACP_TRY(quant(L.wo8, L.s_o, (int)H, qdim_l_));
     if (c.experts > 0) {
       // tensor ids of oracle/synth.py: router = layer_tid(l, 6); expert e: expert_tid(l, e, 0 = [gate; up] | 1 = down)
       ACP_TRY(launch_synth(L.router, (size_t)c.experts * H, c.seed, base + 6, c.w_std, 0, stream_));
       for (int j = 0; j < experts_l_; ++j) {
         const uint32_t etid = (1u << 20) + (uint32_t)l * 256u + (uint32_t)(expert0_ + j) * 2u;
-        SynthMap m = tiled((int)H, (int)H, 0);
-        m.interleave_half = c.ffn;
-        m.seg_global[0] = 0;
-        m.seg_global[1] = c.ffn;
-        ACP_TRY(launch_synth(L.wgu_e + (size_t)j * 2 * c.ffn * H, (size_t)2 * c.ffn * H, c.seed, etid, c.w_std, 0, stream_, m));
-        ACP_TRY(launch_synth(L.wdown_e + (size_t)j * H * c.ffn, H * c.ffn, c.seed, etid + 1, c.w_std, 0, stream_, tiled(c.ffn, c.ffn, 0)));
+        ACP_TRY(launch_synth(L.wgu_e + (size_t)j * 2 * c.ffn * H, (size_t)2 * c.ffn * H, c.seed, etid, c.w_std, 0, stream_, gu_e_map_));
+        ACP_TRY(launch_synth(L.wdown_e + (size_t)j * H * c.ffn, H * c.ffn, c.seed, etid + 1, c.w_std, 0, stream_, down_e_map_));
       }
-    } else {
-      {  // gate/up rows interleaved (2j = gate_j, 2j+1 = up_j); values = oracle's [gate; up] tensor
-        SynthMap m = tiled((int)H, (int)H, 0);
-        m.interleave_half = ffn_l_;
-        m.seg_global[0] = r * ffn_l_;
-        m.seg_global[1] = c.ffn + r * ffn_l_;
-        ACP_TRY(launch_synth(dst(L.wgu), (size_t)2 * ffn_l_ * H, c.seed, base + 2, c.w_std, 0, stream_, m));
-        ACP_TRY(quant(L.wgu8, L.s_gu, 2 * ffn_l_, (int)H));
-      }
-      ACP_TRY(launch_synth(dst(L.wdown), H * ffn_l_, c.seed, base + 3, c.w_std, 0, stream_, tiled(ffn_l_, c.ffn, r * ffn_l_)));
-      ACP_TRY(quant(L.wdown8, L.s_down, (int)H, ffn_l_));
     }
     ACP_TRY(launch_synth(L.attn_norm, H, c.seed, base + 4, 0.1, 1, stream_));
     ACP_TRY(launch_synth(L.ffn_norm, H, c.seed, base + 5, 0.1, 1, stream_));
+    return 0;
+  };
+  int rc = 0;
+  for (int l = 0; l < c.layers && rc == 0; ++l)
+    rc = gen_layer(l);
+  if (stage) {
+    ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    cudaFree(stage);
   }
-  return 0;
+  return rc;
 }
 
 // RoPE tables: same recipe as oracle/llama_oracle.py rope_tables()
@@ -469,25 +416,30 @@ int Model::build_rope_tables() {
 // placed by gather_weight_kernel through the SAME SynthMap the synthetic generator uses.
 int Model::load_weights(const Checkpoint& ck) {
   const ModelConfig& c = cfg_;
-
   const size_t H = c.hidden;
-  const int r = tp_rank_;
-  size_t stage_elems = (size_t)c.qkv_dim() * H;
-  if ((size_t)2 * c.ffn * H > stage_elems) stage_elems = (size_t)2 * c.ffn * H;
-  if ((size_t)lm_rows_l_ * H > stage_elems) stage_elems = (size_t)lm_rows_l_ * H;
+  size_t stage_elems = (size_t)lm_rows_l_ * H, scale_rows = 0;
+  if (c.experts > 0) stage_elems = std::max(stage_elems, (size_t)2 * c.ffn * H);
+  for (const Proj* p : layers_[0].projs()) {
+    size_t rows = 0;
+    for (const Proj::Part& pt : p->parts) rows += pt.rows;
+    stage_elems = std::max(stage_elems, rows * p->map.logical_cols);
+    scale_rows = std::max(scale_rows, rows);
+  }
   __nv_bfloat16* stage = nullptr;
+  float* s_stage = nullptr;   // FP8: the fp32 scale of every logical row
   ACP_CUDA_CHECK(cudaMalloc((void**)&stage, stage_elems * sizeof(__nv_bfloat16)));
+  if (c.fp8) ACP_CUDA_CHECK(cudaMalloc((void**)&s_stage, scale_rows * sizeof(float)));
   std::vector<uint16_t> conv;  // host conversion buffer for F16/F32 checkpoints
-  struct Part { std::string name; int64_t rows, cols; int64_t row0, nrows; };
-  int rc = 0;
-  // copies rows [row0, row0+nrows) of a [rows][cols] tensor to dst (device, bf16)
-  auto upload = [&](const Part& p, __nv_bfloat16* dst) -> int {
-    const StTensor* t = ck.find(p.name);
-    if (!t) { fprintf(stderr, "[acp_infer] checkpoint is missing %s\n", p.name.c_str()); return -1; }
-    const bool shape_ok = p.cols == 1 ? (t->shape.size() == 1 && t->shape[0] == p.rows)
-                                      : (t->shape.size() == 2 && t->shape[0] == p.rows && t->shape[1] == p.cols);
-    if (!shape_ok) { fprintf(stderr, "[acp_infer] %s has an unexpected shape\n", p.name.c_str()); return -1; }
-    const size_t e0 = (size_t)p.row0 * (size_t)p.cols, n = (size_t)p.nrows * (size_t)p.cols;
+  std::vector<float> s_host;
+  // copies rows [row0, row0+nrows) (default: all) of a [rows][cols] tensor to dst (device, bf16)
+  auto upload = [&](const std::string& name, int64_t rows, int64_t cols, __nv_bfloat16* dst, int64_t row0 = 0,
+                    int64_t nrows = -1) -> int {
+    const StTensor* t = ck.find(name);
+    if (!t) { fprintf(stderr, "[acp_infer] checkpoint is missing %s\n", name.c_str()); return -1; }
+    const bool shape_ok = cols == 1 ? (t->shape.size() == 1 && t->shape[0] == rows)
+                                    : (t->shape.size() == 2 && t->shape[0] == rows && t->shape[1] == cols);
+    if (!shape_ok) { fprintf(stderr, "[acp_infer] %s has an unexpected shape\n", name.c_str()); return -1; }
+    const size_t e0 = (size_t)row0 * (size_t)cols, n = (size_t)(nrows < 0 ? rows : nrows) * (size_t)cols;
     if (t->dtype == "BF16") {
       ACP_CUDA_CHECK(cudaMemcpyAsync(dst, t->data + e0 * 2, n * 2, cudaMemcpyHostToDevice, stream_));
       ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
@@ -498,7 +450,7 @@ int Model::load_weights(const Checkpoint& ck) {
     for (size_t o = 0; o < n; o += chunk) {
       const size_t m = n - o < chunk ? n - o : chunk;
       if (!st_to_bf16(*t, e0 + o, m, conv.data())) {
-        fprintf(stderr, "[acp_infer] %s: dtype %s is not supported (BF16, F16, F32)\n", p.name.c_str(), t->dtype.c_str());
+        fprintf(stderr, "[acp_infer] %s: dtype %s is not supported (BF16, F16, F32)\n", name.c_str(), t->dtype.c_str());
         return -1;
       }
       ACP_CUDA_CHECK(cudaMemcpyAsync(dst + o, conv.data(), m * 2, cudaMemcpyHostToDevice, stream_));
@@ -506,150 +458,88 @@ int Model::load_weights(const Checkpoint& ck) {
     }
     return 0;
   };
-  auto tiled = [&](int local_cols, int logical_cols, int col0) {
-    SynthMap m;
-    m.local_cols = local_cols; m.logical_cols = logical_cols; m.col0 = col0;
-    return m;
+  // FP8 (compressed-tensors float-quantized): the F8_E4M3 codes of `<name>` [rows][cols] to dst (device), used
+  // exactly as stored, and its `<name>_scale` (BF16 / F32; [rows, 1] or [rows] per channel, a scalar per tensor,
+  // broadcast to every row) widened to fp32 and appended to s_host
+  auto upload_e4m3 = [&](const std::string& wn, int64_t rows, int64_t cols, uint8_t* dst) -> int {
+    const std::string sn = wn + "_scale";
+    const StTensor* t = ck.find(wn);
+    const StTensor* ts = ck.find(sn);
+    if (!t || !ts) { fprintf(stderr, "[acp_infer] checkpoint is missing %s\n", (!t ? wn : sn).c_str()); return -1; }
+    if (t->dtype != "F8_E4M3" || t->shape.size() != 2 || t->shape[0] != rows || t->shape[1] != cols) {
+      fprintf(stderr, "[acp_infer] %s: expected F8_E4M3 [%lld, %lld]\n", wn.c_str(), (long long)rows, (long long)cols);
+      return -1;
+    }
+    const int64_t ns = ts->numel();
+    const bool per_row = ns == rows && (ts->shape.size() == 1 || (ts->shape.size() == 2 && ts->shape[1] == 1));
+    if ((!per_row && ns != 1) || (ts->dtype != "F32" && ts->dtype != "BF16")) {
+      fprintf(stderr, "[acp_infer] %s: expected a BF16/F32 scale per output row or per tensor\n", sn.c_str());
+      return -1;
+    }
+    for (int64_t r = 0; r < rows; ++r) {
+      const int64_t e = per_row ? r : 0;
+      float v;
+      if (ts->dtype == "F32") memcpy(&v, ts->data + 4 * e, 4);
+      else { uint16_t b; memcpy(&b, ts->data + 2 * e, 2); const uint32_t u = (uint32_t)b << 16; memcpy(&v, &u, 4); }
+      s_host.push_back(v);
+    }
+    ACP_CUDA_CHECK(cudaMemcpyAsync(dst, t->data, t->nbytes, cudaMemcpyHostToDevice, stream_));
+    return 0;
   };
-  auto whole = [&](const std::string& name, int64_t rows, int64_t cols) { return Part{name, rows, cols, 0, rows}; };
-  // FP8 (compressed-tensors float-quantized) projection: the `<name>.weight` F8_E4M3 codes of every part, stacked
-  // row-major in `stage`, and their `<name>.weight_scale` (BF16 / F32; [rows, 1] or [rows] per channel, a scalar
-  // per tensor, broadcast to every row) as fp32; then codes and scales are placed through the bf16 index map.
-  // Codes are used exactly as stored.
-  float* s_stage = nullptr;
-  std::vector<float> s_host;
-  if (c.fp8) {
-    size_t n = (size_t)c.qkv_dim();
-    if ((size_t)2 * c.ffn > n) n = (size_t)2 * c.ffn;
-    if (H > n) n = H;
-    ACP_CUDA_CHECK(cudaMalloc((void**)&s_stage, n * sizeof(float)));
-  }
-  auto upload_fp8 = [&](const std::vector<std::pair<std::string, int64_t>>& parts, int64_t cols, uint8_t* dst,
-                        float* s_dst, int local_rows, const SynthMap& m) -> int {
-    uint8_t* codes = (uint8_t*)stage;
+  // One projection of the layer with name prefix `pre`: the `<stem>.weight` of every part stacked row-major in
+  // `stage` as the logical tensor (bf16, or e4m3 codes + fp32 scales under cfg.fp8), then placed through p.map
+  auto load_proj = [&](const Proj& p, const std::string& pre) -> int {
+    const int64_t cols = p.map.logical_cols;
     int64_t row0 = 0;
     s_host.clear();
-    for (const auto& pr : parts) {
-      const std::string wn = pr.first + ".weight", sn = pr.first + ".weight_scale";
-      const StTensor* t = ck.find(wn);
-      const StTensor* ts = ck.find(sn);
-      if (!t || !ts) { fprintf(stderr, "[acp_infer] checkpoint is missing %s\n", (!t ? wn : sn).c_str()); return -1; }
-      if (t->dtype != "F8_E4M3" || t->shape.size() != 2 || t->shape[0] != pr.second || t->shape[1] != cols) {
-        fprintf(stderr, "[acp_infer] %s: expected F8_E4M3 [%lld, %lld]\n", wn.c_str(), (long long)pr.second, (long long)cols);
-        return -1;
-      }
-      const int64_t ns = ts->numel();
-      const bool per_row = ns == pr.second && (ts->shape.size() == 1 || (ts->shape.size() == 2 && ts->shape[1] == 1));
-      if ((!per_row && ns != 1) || (ts->dtype != "F32" && ts->dtype != "BF16")) {
-        fprintf(stderr, "[acp_infer] %s: expected a BF16/F32 scale per output row or per tensor\n", sn.c_str());
-        return -1;
-      }
-      for (int64_t r = 0; r < pr.second; ++r) {
-        const int64_t e = per_row ? r : 0;
-        float v;
-        if (ts->dtype == "F32") memcpy(&v, ts->data + 4 * e, 4);
-        else { uint16_t b; memcpy(&b, ts->data + 2 * e, 2); const uint32_t u = (uint32_t)b << 16; memcpy(&v, &u, 4); }
-        s_host.push_back(v);
-      }
-      ACP_CUDA_CHECK(cudaMemcpyAsync(codes + (size_t)row0 * cols, t->data, t->nbytes, cudaMemcpyHostToDevice, stream_));
-      row0 += pr.second;
+    for (const Proj::Part& pt : p.parts) {
+      const std::string wn = pre + pt.stem + ".weight";
+      const size_t at = (size_t)row0 * cols;
+      ACP_TRY(c.fp8 ? upload_e4m3(wn, pt.rows, cols, (uint8_t*)stage + at) : upload(wn, pt.rows, cols, stage + at));
+      row0 += pt.rows;
     }
-    ACP_CUDA_CHECK(cudaMemcpyAsync(s_stage, s_host.data(), s_host.size() * sizeof(float), cudaMemcpyHostToDevice, stream_));
-    const size_t n = (size_t)local_rows * (size_t)m.local_cols;
-    int rc2 = launch_gather_weight_e4m3(dst, n, codes, s_dst, local_rows, s_stage, stream_, m);
-    if (rc2 != 0) return rc2;
+    if (c.fp8) {
+      ACP_CUDA_CHECK(cudaMemcpyAsync(s_stage, s_host.data(), s_host.size() * sizeof(float), cudaMemcpyHostToDevice, stream_));
+      ACP_TRY(launch_gather_weight_e4m3(p.codes, (size_t)p.M * p.K, (uint8_t*)stage, p.scale, p.M, s_stage, stream_, p.map));
+    } else {
+      ACP_TRY(launch_gather_weight(p.w, (size_t)p.M * p.K, stage, 0, stream_, p.map));
+    }
     ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
     return 0;
   };
-  do {
-    if ((rc = upload(whole("model.embed_tokens.weight", c.vocab, H), embed_)) != 0) break;
-    {  // LM head: this shard's rows only (contiguous in the logical tensor)
-      const bool tied = c.tied_embeddings || !ck.find("lm_head.weight");
-      Part p{tied ? "model.embed_tokens.weight" : "lm_head.weight", c.vocab, (int64_t)H, lm_row0_, lm_rows_l_};
-      if ((rc = upload(p, stage)) != 0) break;
-      SynthMap m = tiled((int)H, (int)H, 0);
-      m.nseg = 1; m.seg_rows[0] = lm_rows_l_; m.seg_global[0] = lm_row0_;
-      if ((rc = launch_gather_weight(lm_head_, (size_t)lm_rows_l_ * H, stage, (size_t)lm_row0_ * H, stream_, m)) != 0) break;
-      ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    }
-    if ((rc = upload(whole("model.norm.weight", H, 1), final_norm_)) != 0) break;
-    for (int l = 0; l < c.layers && rc == 0; ++l) {
+  auto load_all = [&]() -> int {
+    ACP_TRY(upload("model.embed_tokens.weight", c.vocab, H, embed_));
+    // LM head: this shard's rows only
+    const bool tied = c.tied_embeddings || !ck.find("lm_head.weight");
+    ACP_TRY(upload(tied ? "model.embed_tokens.weight" : "lm_head.weight", c.vocab, H, stage, lm_row0_, lm_rows_l_));
+    ACP_TRY(launch_gather_weight(lm_head_, (size_t)lm_rows_l_ * H, stage, (size_t)lm_row0_ * H, stream_, lm_map_));
+    ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    ACP_TRY(upload("model.norm.weight", H, 1, final_norm_));
+    for (int l = 0; l < c.layers; ++l) {
       Layer& L = layers_[l];
       const std::string pre = "model.layers." + std::to_string(l) + ".";
-      if (c.fp8) {
-        SynthMap m = tiled((int)H, (int)H, 0);
-        m.nseg = 3;
-        m.seg_rows[0] = qdim_l_; m.seg_global[0] = r * qdim_l_;
-        m.seg_rows[1] = kvdim_l_; m.seg_global[1] = c.q_dim() + r * kvdim_l_;
-        m.seg_rows[2] = kvdim_l_; m.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
-        if ((rc = upload_fp8({{pre + "self_attn.q_proj", c.q_dim()}, {pre + "self_attn.k_proj", c.kv_dim()}, {pre + "self_attn.v_proj", c.kv_dim()}},
-                             H, L.wqkv8, L.s_qkv, qkv_l_, m)) != 0) break;
-        if ((rc = upload_fp8({{pre + "self_attn.o_proj", H}}, c.q_dim(), L.wo8, L.s_o, (int)H, tiled(qdim_l_, c.q_dim(), r * qdim_l_))) != 0) break;
-        m = tiled((int)H, (int)H, 0);
-        m.interleave_half = ffn_l_;
-        m.seg_global[0] = r * ffn_l_;
-        m.seg_global[1] = c.ffn + r * ffn_l_;
-        if ((rc = upload_fp8({{pre + "mlp.gate_proj", c.ffn}, {pre + "mlp.up_proj", c.ffn}}, H, L.wgu8, L.s_gu, 2 * ffn_l_, m)) != 0) break;
-        if ((rc = upload_fp8({{pre + "mlp.down_proj", H}}, c.ffn, L.wdown8, L.s_down, (int)H, tiled(ffn_l_, c.ffn, r * ffn_l_))) != 0) break;
-        if ((rc = upload(whole(pre + "input_layernorm.weight", H, 1), L.attn_norm)) != 0) break;
-        if ((rc = upload(whole(pre + "post_attention_layernorm.weight", H, 1), L.ffn_norm)) != 0) break;
-        continue;
-      }
-      {  // logical [q; k; v]
-        if ((rc = upload(whole(pre + "self_attn.q_proj.weight", c.q_dim(), H), stage)) != 0) break;
-        if ((rc = upload(whole(pre + "self_attn.k_proj.weight", c.kv_dim(), H), stage + (size_t)c.q_dim() * H)) != 0) break;
-        if ((rc = upload(whole(pre + "self_attn.v_proj.weight", c.kv_dim(), H), stage + (size_t)(c.q_dim() + c.kv_dim()) * H)) != 0) break;
-        SynthMap m = tiled((int)H, (int)H, 0);
-        m.nseg = 3;
-        m.seg_rows[0] = qdim_l_; m.seg_global[0] = r * qdim_l_;
-        m.seg_rows[1] = kvdim_l_; m.seg_global[1] = c.q_dim() + r * kvdim_l_;
-        m.seg_rows[2] = kvdim_l_; m.seg_global[2] = c.q_dim() + c.kv_dim() + r * kvdim_l_;
-        if ((rc = launch_gather_weight(L.wqkv, (size_t)qkv_l_ * H, stage, 0, stream_, m)) != 0) break;
-        ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-      }
-      if ((rc = upload(whole(pre + "self_attn.o_proj.weight", H, c.q_dim()), stage)) != 0) break;
-      if ((rc = launch_gather_weight(L.wo, H * qdim_l_, stage, 0, stream_, tiled(qdim_l_, c.q_dim(), r * qdim_l_))) != 0) break;
-      ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
+      for (const Proj* p : L.projs()) ACP_TRY(load_proj(*p, pre));
       if (c.experts > 0) {
         // Mixtral (hub layout): block_sparse_moe.gate.weight [E][H]; experts.<e>.w1 = gate, w3 = up ([ffn][H]), w2 = down ([H][ffn])
         const std::string moe = pre + "block_sparse_moe.";
-        if ((rc = upload(whole(moe + "gate.weight", c.experts, H), L.router)) != 0) break;
-        for (int j = 0; j < experts_l_ && rc == 0; ++j) {
+        ACP_TRY(upload(moe + "gate.weight", c.experts, H, L.router));
+        for (int j = 0; j < experts_l_; ++j) {
           const std::string ex = moe + "experts." + std::to_string(expert0_ + j) + ".";
-          if ((rc = upload(whole(ex + "w1.weight", c.ffn, H), stage)) != 0) break;
-          if ((rc = upload(whole(ex + "w3.weight", c.ffn, H), stage + (size_t)c.ffn * H)) != 0) break;
-          SynthMap m = tiled((int)H, (int)H, 0);
-          m.interleave_half = c.ffn;
-          m.seg_global[0] = 0;
-          m.seg_global[1] = c.ffn;
-          if ((rc = launch_gather_weight(L.wgu_e + (size_t)j * 2 * c.ffn * H, (size_t)2 * c.ffn * H, stage, 0, stream_, m)) != 0) break;
+          ACP_TRY(upload(ex + "w1.weight", c.ffn, H, stage));
+          ACP_TRY(upload(ex + "w3.weight", c.ffn, H, stage + (size_t)c.ffn * H));
+          ACP_TRY(launch_gather_weight(L.wgu_e + (size_t)j * 2 * c.ffn * H, (size_t)2 * c.ffn * H, stage, 0, stream_, gu_e_map_));
           ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-          if ((rc = upload(whole(ex + "w2.weight", H, c.ffn), stage)) != 0) break;
-          if ((rc = launch_gather_weight(L.wdown_e + (size_t)j * H * c.ffn, H * c.ffn, stage, 0, stream_, tiled(c.ffn, c.ffn, 0))) != 0) break;
+          ACP_TRY(upload(ex + "w2.weight", H, c.ffn, stage));
+          ACP_TRY(launch_gather_weight(L.wdown_e + (size_t)j * H * c.ffn, H * c.ffn, stage, 0, stream_, down_e_map_));
           ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
         }
-        if (rc != 0) break;
-        if ((rc = upload(whole(pre + "input_layernorm.weight", H, 1), L.attn_norm)) != 0) break;
-        if ((rc = upload(whole(pre + "post_attention_layernorm.weight", H, 1), L.ffn_norm)) != 0) break;
-        continue;
       }
-      {  // logical [gate; up], stored interleaved (2j = gate_j, 2j+1 = up_j)
-        if ((rc = upload(whole(pre + "mlp.gate_proj.weight", c.ffn, H), stage)) != 0) break;
-        if ((rc = upload(whole(pre + "mlp.up_proj.weight", c.ffn, H), stage + (size_t)c.ffn * H)) != 0) break;
-        SynthMap m = tiled((int)H, (int)H, 0);
-        m.interleave_half = ffn_l_;
-        m.seg_global[0] = r * ffn_l_;
-        m.seg_global[1] = c.ffn + r * ffn_l_;
-        if ((rc = launch_gather_weight(L.wgu, (size_t)2 * ffn_l_ * H, stage, 0, stream_, m)) != 0) break;
-        ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-      }
-      if ((rc = upload(whole(pre + "mlp.down_proj.weight", H, c.ffn), stage)) != 0) break;
-      if ((rc = launch_gather_weight(L.wdown, H * ffn_l_, stage, 0, stream_, tiled(ffn_l_, c.ffn, r * ffn_l_))) != 0) break;
-      ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-      if ((rc = upload(whole(pre + "input_layernorm.weight", H, 1), L.attn_norm)) != 0) break;
-      if ((rc = upload(whole(pre + "post_attention_layernorm.weight", H, 1), L.ffn_norm)) != 0) break;
+      ACP_TRY(upload(pre + "input_layernorm.weight", H, 1, L.attn_norm));
+      ACP_TRY(upload(pre + "post_attention_layernorm.weight", H, 1, L.ffn_norm));
     }
-  } while (false);
+    return 0;
+  };
+  const int rc = load_all();
   cudaFree(stage);
   if (s_stage) cudaFree(s_stage);
   return rc;
@@ -673,41 +563,43 @@ StepInput& Model::stage_begin(int T, int B, int n_blocks) {
   return s;
 }
 
-int Model::gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out,
-                const float* w_scale, const float* x_scale) {
+// One launch of p's GEMM over N rows of a into `out` (leading dimension ld)
+int Model::launch_proj(const Proj& p, const Act& a, int N, int epi, int splits, void* out, int ld) {
   GemmLaunch g;
   g.tp_shard = tp_size_ > 1;
-  g.w = &w.w; g.x = &x; g.M = M; g.N = N; g.K = K;
-  g.fp8 = cfg_.fp8; g.w_scale = w_scale; g.x_scale = x_scale;
-  const int splits = choose_splits(M, K, N);
-  if (decode && splits > 1) {  // a single split writes bf16 directly (same rounding, half the bytes)
-    g.epi = EPI_F32; g.splits = splits; g.out = ws_; g.ld = M; g.n_cap = N;
-    if ((size_t)splits * N * M * sizeof(float) > ws_bytes_) { fprintf(stderr, "[acp_infer] split-K workspace too small: %d planes x %d x %d\n", splits, N, M); return -4; }
-    out->ptr = ws_; out->splits = splits; out->n_cap = N; out->ld = M;
-  } else {
-    g.epi = EPI_BF16; g.splits = 1; g.out = gemm_bf16_; g.ld = M; g.n_cap = N;
-    out->ptr = gemm_bf16_; out->splits = 0; out->n_cap = N; out->ld = M;
+  g.w = &p.m.w; g.x = &a.m; g.M = p.M; g.N = N; g.K = p.K;
+  g.epi = epi; g.splits = splits; g.out = out; g.ld = ld; g.n_cap = N;
+  if (cfg_.fp8) { g.fp8 = true; g.w_scale = p.scale; g.x_scale = a.scale; }
+  if (out == ws_ && (size_t)splits * N * p.M * sizeof(float) > ws_bytes_) {
+    fprintf(stderr, "[acp_infer] split-K workspace too small: %d planes x %d x %d\n", splits, N, p.M);
+    return -4;
   }
   ++launches_;
   return gemm_launch(g, stream_);
 }
 
-int Model::quantize_act(const __nv_bfloat16* x, int T, int cols, uint8_t* codes, float* scales) {
-  ++launches_;
-  return launch_quantize_rows_e4m3(x, T, cols, codes, scales, stream_);
+int Model::gemm(const char* name, const Proj& p, const Act& a, int T, bool decode, GemmOut* out, bool swiglu) {
+  if (cfg_.fp8) {   // the activation's columns are p's K
+    PROF(a.quant, launch_quantize_rows_e4m3(a.x, T, p.K, a.x8, a.scale, stream_));
+    ++launches_;
+  }
+  if (swiglu) {
+    PROF(name, launch_proj(p, a, T, EPI_SWIGLU, 1, h_.x, p.M / 2));
+    return 0;
+  }
+  const int splits = choose_splits(p.M, p.K, T);
+  const bool planes = decode && splits > 1;   // a single split writes bf16 directly (same rounding, half the bytes)
+  *out = planes ? GemmOut{ws_, splits, T, p.M} : GemmOut{gemm_bf16_, 0, T, p.M};
+  PROF(name, launch_proj(p, a, T, planes ? EPI_F32 : EPI_BF16, planes ? splits : 1, (void*)out->ptr, p.M));
+  return 0;
 }
 
 // Row-parallel GEMM of a tensor-parallel shard (O and down projections): fp32 partial sums, local
 // split-K reduce, NCCL all-reduce (sum) across the group over NVLink, consumer rounds to bf16 ONCE.
-int Model::gemm_rowpar(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out) {
-  GemmLaunch g;
-  g.tp_shard = tp_size_ > 1;
-  g.w = &w.w; g.x = &x; g.M = M; g.N = N; g.K = K;
-  const int splits = decode ? choose_splits(M, K, N) : 1;
-  g.epi = EPI_F32; g.splits = splits; g.out = ws_; g.ld = M; g.n_cap = N;
-  if ((size_t)splits * N * M * sizeof(float) > ws_bytes_) { fprintf(stderr, "[acp_infer] split-K workspace too small: %d planes x %d x %d\n", splits, N, M); return -4; }
-  ++launches_;
-  int rc = gemm_launch(g, stream_);
+int Model::gemm_rowpar(const Proj& p, const Act& a, int N, bool decode, GemmOut* out) {
+  const int M = p.M;
+  const int splits = decode ? choose_splits(M, p.K, N) : 1;
+  int rc = launch_proj(p, a, N, EPI_F32, splits, ws_, M);
   if (rc != 0) return rc;
   float* ar = ws_;
   if (splits > 1) {
@@ -727,19 +619,11 @@ int Model::gemm_rowpar(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, 
 // Row-parallel GEMM + the fused peer-memory exchange of tp_comm.cu:
 //   GEMM (fp32 partial planes) -> local split-K reduce -> barrier -> pull/reduce/residual/RMSNorm/
 //   push -> barrier.  x_ and xn_ are updated on EVERY rank by the rank that owns the row.
-int Model::rowpar_fused(const TmaMaps& w, const TmaMaps& x, int K, int N, bool decode, const __nv_bfloat16* gain,
-                        bool push_x) {
-  const int M = cfg_.hidden;
-  GemmLaunch g;
-  g.tp_shard = tp_size_ > 1;
-  g.w = &w.w; g.x = &x; g.M = M; g.N = N; g.K = K;
-  const int splits = decode ? choose_splits(M, K, N) : 1;
-  g.epi = EPI_F32; g.splits = splits; g.ld = M; g.n_cap = N;
-  g.out = splits > 1 ? ws_ : ar_buf_;
-  if (splits > 1 && (size_t)splits * N * M * sizeof(float) > ws_bytes_) { fprintf(stderr, "[acp_infer] split-K workspace too small: %d planes x %d x %d\n", splits, N, M); return -4; }
-  int rc = gemm_launch(g, stream_);
+int Model::rowpar_fused(const Proj& p, const Act& a, int N, bool decode, const __nv_bfloat16* gain, bool push_x) {
+  const int M = p.M;
+  const int splits = decode ? choose_splits(M, p.K, N) : 1;
+  int rc = launch_proj(p, a, N, EPI_F32, splits, splits > 1 ? ws_ : ar_buf_, M);
   if (rc != 0) return rc;
-  ++launches_;
   if (splits > 1) {
     rc = launch_reduce_planes(ws_, splits, (size_t)N * M, ar_buf_, stream_);
     if (rc != 0) return rc;
@@ -807,19 +691,14 @@ int Model::forward(const StepInput& in) {
   PROF("embed", launch_embed(d_tok, embed_, x_, T, c.hidden, stream_));
   ++launches_;
   GemmOut none;
-  PROF("rmsnorm_first", launch_add_rmsnorm(x_, none, layers_[0].attn_norm, xn_, nullptr, T, c.hidden, c.eps, stream_));
+  PROF("rmsnorm_first", launch_add_rmsnorm(x_, none, layers_[0].attn_norm, xn_.x, nullptr, T, c.hidden, c.eps, stream_));
   ++launches_;
   for (int l = 0; l < c.layers; ++l) {
     Layer& L = layers_[l];
     GemmOut qkv, o, dn;
     // investigation knob (ACP_TP_SYNC_EVERY): bound this shard's launch queue
     if (tp_sync_every_ > 0 && l > 0 && l % tp_sync_every_ == 0) ACP_CUDA_CHECK(cudaStreamSynchronize(stream_));
-    if (c.fp8) {
-      PROF("quant_xn", quantize_act(xn_, T, c.hidden, xn8_, sx_xn_));
-      PROF("gemm_qkv", gemm(L.m_qkv, m_xn8_, qkv_l_, c.hidden, T, in.decode, &qkv, L.s_qkv, sx_xn_));
-    } else {
-      PROF("gemm_qkv", gemm(L.m_qkv, m_xn_, qkv_l_, c.hidden, T, in.decode, &qkv));
-    }
+    ACP_TRY(gemm("gemm_qkv", L.qkv, xn_, T, in.decode, &qkv));
     if (!in.decode) {
       RopeKvArgs ra;
       ra.qkv = qkv; ra.pos = d_pos; ra.seq_of_row = d_seq; ra.page_table = d_pt;
@@ -830,7 +709,7 @@ int Model::forward(const StepInput& in) {
     }
     if (in.decode) {
       AttnDecodeArgs aa;
-      aa.q = qbuf_; aa.out = attn_; aa.ctx_len = d_ctx; aa.chunk_cum = dev(in.tile_cum); aa.page_table = d_pt;
+      aa.q = qbuf_; aa.out = attn_.x; aa.ctx_len = d_ctx; aa.chunk_cum = dev(in.tile_cum); aa.page_table = d_pt;
       aa.max_pages = lim_.max_pages_per_seq; aa.heads = heads_l_; aa.kv_heads = kvh_l_;
       aa.num_seqs = in.B;
       aa.total_chunks = in.tile_cum[in.B];   // host copy of the prefix sum (filled by the engine)
@@ -848,7 +727,7 @@ int Model::forward(const StepInput& in) {
       launches_ += aa.per_item ? 1 : 2;
     } else {
       AttnPrefillArgs pa;
-      pa.q = qbuf_; pa.out = attn_; pa.blk_seq = d_bseq; pa.blk_tok0 = d_btok0; pa.q_start = d_qstart;
+      pa.q = qbuf_; pa.out = attn_.x; pa.blk_seq = d_bseq; pa.blk_tok0 = d_btok0; pa.q_start = d_qstart;
       pa.q_len = d_qlen; pa.ctx_len = d_ctx; pa.page_table = d_pt; pa.max_pages = lim_.max_pages_per_seq;
       pa.heads = heads_l_; pa.kv_heads = kvh_l_; pa.scale = scale;
       if (attn_prefill_tc_enabled()) PROF("attn_prefill", launch_attn_prefill_tc(tm_q_, L.tm_k32, L.tm_v32, pa, in.n_blocks, stream_));
@@ -856,14 +735,11 @@ int Model::forward(const StepInput& in) {
       ++launches_;
     }
     if (tp_size_ > 1 && have_peers_) {
-      PROF("gemm_o+p2p_allreduce_norm", rowpar_fused(L.m_o, m_attn_, qdim_l_, T, in.decode, L.ffn_norm, false));
+      PROF("gemm_o+p2p_allreduce_norm", rowpar_fused(L.o, attn_, T, in.decode, L.ffn_norm, false));
     } else {
-      if (tp_size_ > 1) PROF("gemm_o_allreduce", gemm_rowpar(L.m_o, m_attn_, c.hidden, qdim_l_, T, in.decode, &o));
-      else if (c.fp8) {
-        PROF("quant_attn", quantize_act(attn_, T, qdim_l_, attn8_, sx_attn_));
-        PROF("gemm_o", gemm(L.m_o, m_attn8_, c.hidden, qdim_l_, T, in.decode, &o, L.s_o, sx_attn_));
-      } else PROF("gemm_o", gemm(L.m_o, m_attn_, c.hidden, qdim_l_, T, in.decode, &o));
-      PROF("add_rmsnorm_o", launch_add_rmsnorm(x_, o, L.ffn_norm, xn_, nullptr, T, c.hidden, c.eps, stream_));
+      if (tp_size_ > 1) PROF("gemm_o_allreduce", gemm_rowpar(L.o, attn_, T, in.decode, &o));
+      else ACP_TRY(gemm("gemm_o", L.o, attn_, T, in.decode, &o));
+      PROF("add_rmsnorm_o", launch_add_rmsnorm(x_, o, L.ffn_norm, xn_.x, nullptr, T, c.hidden, c.eps, stream_));
       ++launches_;
     }
     if (c.experts > 0) {
@@ -877,28 +753,20 @@ int Model::forward(const StepInput& in) {
       }
       continue;
     }
-    if (c.fp8) PROF("quant_xn", quantize_act(xn_, T, c.hidden, xn8_, sx_xn_));
-    if (fuse_swiglu_ || (!in.decode && T > 256 && fuse_swiglu_prefill_)) {
-      // SwiGLU in the GEMM epilogue.  Decode (non-persistent kernel, epilogue exposed at the end of
-      // every CTA) measured no gain, so it stays a separate kernel there unless ACP_FUSE_SWIGLU=1.
-      GemmLaunch g;
-      g.tp_shard = tp_size_ > 1;
-      g.w = &L.m_gu.w; g.x = &m_xn_; g.M = 2 * ffn_l_; g.N = T; g.K = c.hidden; g.splits = 1;
-      g.epi = EPI_SWIGLU; g.out = h_; g.ld = ffn_l_; g.n_cap = T;
-      if (c.fp8) { g.fp8 = true; g.x = &m_xn8_; g.w_scale = L.s_gu; g.x_scale = sx_xn_; }
-      PROF("gemm_gateup_swiglu", gemm_launch(g, stream_));
-      ++launches_;
+    if (!in.decode && T > 256) {
+      // prefill: SwiGLU in the persistent gate/up GEMM's epilogue, overlapped with the next tile.  Decode
+      // (non-persistent kernel, epilogue exposed at the end of every CTA) measured no gain from fusing.
+      ACP_TRY(gemm("gemm_gateup_swiglu", L.gu, xn_, T, in.decode, nullptr, true));
     } else {
       GemmOut gu;
-      if (c.fp8) PROF("gemm_gateup", gemm(L.m_gu, m_xn8_, 2 * ffn_l_, c.hidden, T, in.decode, &gu, L.s_gu, sx_xn_));
-      else PROF("gemm_gateup", gemm(L.m_gu, m_xn_, 2 * ffn_l_, c.hidden, T, in.decode, &gu));
-      PROF("swiglu", launch_swiglu(gu, h_, T, ffn_l_, stream_));
+      ACP_TRY(gemm("gemm_gateup", L.gu, xn_, T, in.decode, &gu));
+      PROF("swiglu", launch_swiglu(gu, h_.x, T, ffn_l_, stream_));
       ++launches_;
     }
     if (tp_size_ > 1 && have_peers_) {
       // fused exchange writes x_ and xn_ (with the next layer's gain; the last layer's xn_ is unused)
       const __nv_bfloat16* gain = (l + 1 < c.layers) ? layers_[l + 1].attn_norm : final_norm_;
-      PROF("gemm_down+p2p_allreduce_norm", rowpar_fused(L.m_down, m_h_, ffn_l_, T, in.decode, gain, l + 1 == c.layers));
+      PROF("gemm_down+p2p_allreduce_norm", rowpar_fused(L.down, h_, T, in.decode, gain, l + 1 == c.layers));
       if (l + 1 == c.layers) {
         GemmOut nothing;
         PROF("add_rmsnorm_final", launch_add_rmsnorm(x_, nothing, final_norm_, xs_, d_srows, in.n_sample, c.hidden, c.eps, stream_));
@@ -906,13 +774,10 @@ int Model::forward(const StepInput& in) {
       }
       continue;
     }
-    if (tp_size_ > 1) PROF("gemm_down_allreduce", gemm_rowpar(L.m_down, m_h_, c.hidden, ffn_l_, T, in.decode, &dn));
-    else if (c.fp8) {
-      PROF("quant_h", quantize_act(h_, T, ffn_l_, h8_, sx_h_));
-      PROF("gemm_down", gemm(L.m_down, m_h8_, c.hidden, ffn_l_, T, in.decode, &dn, L.s_down, sx_h_));
-    } else PROF("gemm_down", gemm(L.m_down, m_h_, c.hidden, ffn_l_, T, in.decode, &dn));
+    if (tp_size_ > 1) PROF("gemm_down_allreduce", gemm_rowpar(L.down, h_, T, in.decode, &dn));
+    else ACP_TRY(gemm("gemm_down", L.down, h_, T, in.decode, &dn));
     if (l + 1 < c.layers) {
-      PROF("add_rmsnorm_down", launch_add_rmsnorm(x_, dn, layers_[l + 1].attn_norm, xn_, nullptr, T, c.hidden, c.eps, stream_));
+      PROF("add_rmsnorm_down", launch_add_rmsnorm(x_, dn, layers_[l + 1].attn_norm, xn_.x, nullptr, T, c.hidden, c.eps, stream_));
     } else {
       // final norm only on the rows that are sampled (residual add folded in, not written back)
       PROF("add_rmsnorm_final", launch_add_rmsnorm(x_, dn, final_norm_, xs_, d_srows, in.n_sample, c.hidden, c.eps, stream_));
@@ -983,11 +848,11 @@ int Model::forward(const StepInput& in) {
 // The expert GEMMs never split K (prefill and decode share one arithmetic path).
 int Model::moe_mlp(Layer& L, int T, const __nv_bfloat16* gain, bool last_layer) {
   const ModelConfig& c = cfg_;
-  PROF("moe_router", launch_moe_router(xn_, L.router, c.hidden, c.experts, T, moe_topk_idx_, moe_topk_w_, stream_));
+  PROF("moe_router", launch_moe_router(xn_.x, L.router, c.hidden, c.experts, T, moe_topk_idx_, moe_topk_w_, stream_));
   // N tile of the expert GEMMs: an expert sees about 2T / E rows (a token picks an expert at most once)
   const int bn = gemm_pick_bn((2 * T + c.experts - 1) / c.experts);
   PROF("moe_dispatch", launch_moe_dispatch(moe_topk_idx_, T, expert0_, experts_l_, bn, moe_ranges_, moe_row_of_, stream_));
-  PROF("moe_gather", launch_moe_gather(xn_, moe_row_of_, c.hidden, T, xe_, stream_));
+  PROF("moe_gather", launch_moe_gather(xn_.x, moe_row_of_, c.hidden, T, xe_, stream_));
   GemmLaunch g;
   g.tp_shard = tp_size_ > 1;
   g.groups = experts_l_; g.group_ranges = moe_ranges_; g.splits = 1;
@@ -1014,7 +879,7 @@ int Model::moe_mlp(Layer& L, int T, const __nv_bfloat16* gain, bool last_layer) 
       if (rc != 0) { fprintf(stderr, "[acp_infer] ncclAllReduce: %s\n", nc.GetErrorString(rc)); return -5; }
       GemmOut o;
       o.ptr = ar_buf_; o.splits = 1; o.n_cap = T; o.ld = c.hidden;
-      PROF("add_rmsnorm_moe", launch_add_rmsnorm(x_, o, gain, xn_, nullptr, T, c.hidden, c.eps, stream_));
+      PROF("add_rmsnorm_moe", launch_add_rmsnorm(x_, o, gain, xn_.x, nullptr, T, c.hidden, c.eps, stream_));
       launches_ += 2;
     }
     return 0;
@@ -1022,7 +887,7 @@ int Model::moe_mlp(Layer& L, int T, const __nv_bfloat16* gain, bool last_layer) 
   PROF("moe_combine", launch_moe_combine(ye_, moe_row_of_, moe_topk_w_, c.hidden, T, gemm_bf16_, false, stream_));
   GemmOut o;
   o.ptr = gemm_bf16_; o.splits = 0; o.n_cap = T; o.ld = c.hidden;
-  PROF("add_rmsnorm_moe", launch_add_rmsnorm(x_, o, gain, xn_, nullptr, T, c.hidden, c.eps, stream_));
+  PROF("add_rmsnorm_moe", launch_add_rmsnorm(x_, o, gain, xn_.x, nullptr, T, c.hidden, c.eps, stream_));
   launches_ += 2;
   return 0;
 }

@@ -85,28 +85,21 @@ class Model {
   void set_peers(const TpPeers& p) { peers_ = p; have_peers_ = true; }
   float* ar_buffer() const { return ar_buf_; }
   __nv_bfloat16* x_buffer() const { return x_; }
-  __nv_bfloat16* xn_buffer() const { return xn_; }
+  __nv_bfloat16* xn_buffer() const { return xn_.x; }
   int* tp_flags() const { return tp_flags_; }
 
  private:
   int alloc_all();
   int gen_weights();
-  int gen_layer_weights(int l, __nv_bfloat16* stage);
   int load_weights(const Checkpoint& ck);   // HuggingFace Llama safetensors -> tiled/sharded HBM layout
   int build_rope_tables();
-  // w_scale / x_scale: the FP8 presets' scales (w and x are then e4m3 maps)
-  int gemm(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out,
-           const float* w_scale = nullptr, const float* x_scale = nullptr);
-  int quantize_act(const __nv_bfloat16* x, int T, int cols, uint8_t* codes, float* scales);
   int choose_splits(int M, int K, int N) const;
-  int gemm_rowpar(const TmaMaps& w, const TmaMaps& x, int M, int K, int N, bool decode, GemmOut* out);
 
   ModelConfig cfg_;
   ModelLimits lim_;
   int device_ = 0;
   cudaStream_t stream_ = nullptr;
   long long launches_ = 0, h2d_bytes_ = 0, d2h_bytes_ = 0;
-  bool fuse_swiglu_ = false, fuse_swiglu_prefill_ = false;
   int tp_sync_every_ = 0;   // ACP_TP_SYNC_EVERY=n (tensor-parallel engines only): stream synchronize every n layers
   // tensor parallel
   int tp_rank_ = 0, tp_size_ = 1;
@@ -125,36 +118,57 @@ class Model {
   bool have_peers_ = false;
   int* tp_flags_ = nullptr;
   int tp_epoch_ = 0;
-  int rowpar_fused(const TmaMaps& w, const TmaMaps& x, int K, int N, bool decode, const __nv_bfloat16* gain,
-                   bool push_x);
+  // One dense projection of a layer (QKV, O, gate/up, down): this shard's M x K weight, where it sits in the
+  // logical tensor that oracle/synth.py generates and a checkpoint stores, and its storage.
+  struct Proj {
+    struct Part { const char* stem; int rows; };   // checkpoint tensor `<stem>.weight` of the layer
+    int M = 0, K = 0;
+    SynthMap map;
+    uint32_t tid = 0;               // synthetic tensor id: the layer's base + tid
+    std::vector<Part> parts;        // stacked row-wise into the logical tensor, e.g. [q; k; v]
+    __nv_bfloat16* w = nullptr;     // bf16 tiles
+    uint8_t* codes = nullptr;       // cfg.fp8 instead: e4m3 tiles and one fp32 scale per row
+    float* scale = nullptr;
+    TmaMaps m;
+  };
+  // An activation a projection reads, [rows][cols] row-major; under cfg.fp8 also its e4m3 copy and per-token scales
+  struct Act {
+    __nv_bfloat16* x = nullptr;
+    uint8_t* x8 = nullptr;
+    float* scale = nullptr;
+    TmaMaps m;                      // what the GEMM reads: over x, or over x8 under cfg.fp8
+    const char* quant = nullptr;    // profile name of its quantiser
+  };
+  void describe_weights();   // the layout of every projection, the LM head and the experts
+  int alloc_proj(Proj& p);
+  int alloc_act(Act& a, int rows, int cols, const char* quant);
+  int launch_proj(const Proj& p, const Act& a, int N, int epi, int splits, void* out, int ld);
+  // `name`: the GEMM's profile segment.  Quantises `a` first under cfg.fp8; swiglu: gate/up into h_
+  int gemm(const char* name, const Proj& p, const Act& a, int T, bool decode, GemmOut* out, bool swiglu = false);
+  int gemm_rowpar(const Proj& p, const Act& a, int N, bool decode, GemmOut* out);
+  int rowpar_fused(const Proj& p, const Act& a, int N, bool decode, const __nv_bfloat16* gain, bool push_x);
 
   struct Layer {
-    __nv_bfloat16 *wqkv, *wo, *wgu, *wdown, *attn_norm, *ffn_norm;
+    Proj qkv, o, gu, down;          // gu, down: dense layers only (M == 0 otherwise)
+    std::vector<Proj*> projs() { return gu.M ? std::vector<Proj*>{&qkv, &o, &gu, &down} : std::vector<Proj*>{&qkv, &o}; }
+    __nv_bfloat16 *attn_norm, *ffn_norm;
     // mixture of experts (cfg.experts > 0): router [E][hidden] row-major; this rank's experts concatenated,
     // each tiled like the dense matrices: wgu_e [E_l][2 ffn][hidden] (gate/up rows interleaved), wdown_e [E_l][hidden][ffn]
     __nv_bfloat16 *router = nullptr, *wgu_e = nullptr, *wdown_e = nullptr;
     TmaMaps m_gu_e, m_down_e;
     __nv_bfloat16 *k_cache, *v_cache;
-    TmaMaps m_qkv, m_o, m_gu, m_down;   // over the e4m3 copies below when cfg.fp8
-    // FP8 presets: tiled e4m3 codes of the four projections (same row order as the bf16 matrices, which
-    // are then never allocated) and their fp32 per-row scales
-    uint8_t *wqkv8 = nullptr, *wo8 = nullptr, *wgu8 = nullptr, *wdown8 = nullptr;
-    float *s_qkv = nullptr, *s_o = nullptr, *s_gu = nullptr, *s_down = nullptr;
     CUtensorMap tm_k, tm_v;       // box = one (page, kv head) block, both dim halves (decode kernels)
     CUtensorMap tm_k32, tm_v32;   // box = one dim half of a page (wgmma prefill kernel)
   };
   std::vector<Layer> layers_;
   __nv_bfloat16 *embed_ = nullptr, *lm_head_ = nullptr, *final_norm_ = nullptr;
   TmaMaps m_lm_;
+  SynthMap lm_map_, gu_e_map_, down_e_map_;   // LM head rows of this shard; one expert's [gate; up] and down
   float *cos_ = nullptr, *sin_ = nullptr;
   // activations
-  __nv_bfloat16 *x_ = nullptr, *xn_ = nullptr, *qbuf_ = nullptr, *attn_ = nullptr, *h_ = nullptr,
-                *xs_ = nullptr, *gemm_bf16_ = nullptr;
-  TmaMaps m_xn_, m_attn_, m_h_, m_xs_;
-  // FP8 presets: e4m3 copies of xn / attn / h (row-major) and their per-token scales
-  uint8_t *xn8_ = nullptr, *attn8_ = nullptr, *h8_ = nullptr;
-  float *sx_xn_ = nullptr, *sx_attn_ = nullptr, *sx_h_ = nullptr;
-  TmaMaps m_xn8_, m_attn8_, m_h8_;
+  __nv_bfloat16 *x_ = nullptr, *qbuf_ = nullptr, *xs_ = nullptr, *gemm_bf16_ = nullptr;
+  Act xn_, attn_, h_;   // h_: dense layers only
+  TmaMaps m_xs_;
   CUtensorMap tm_q_;   // qbuf_ as {128 dims, heads, rows} for the prefill attention's Q tiles
   float* ws_ = nullptr;  // split-K partial planes
   size_t ws_bytes_ = 0;

@@ -67,16 +67,23 @@ def test_checkpoint_tensor_parallel(tmp_path, prompts, synthetic):
 
 
 def test_missing_tensor_fails_init(tmp_path):
+    """A checkpoint missing one tensor is refused at init: a bf16 weight, or an FP8 projection's weight_scale."""
     import os
     from safetensors.torch import load_file, save_file
-    d = str(tmp_path / "broken")
-    write_checkpoint(d, PRESETS["tiny"], SEED)
-    f = os.path.join(d, "model.safetensors")
-    t = load_file(f)
-    del t["model.layers.1.mlp.down_proj.weight"]
-    save_file(t, f)
-    with pytest.raises(RuntimeError):
-        Engine(dict(BASE, weights=d))
+    from fp8_ckpt_util import write_fp8_checkpoint
+    from oracle.fp8 import FP8_PRESETS
+    for name, write, missing in (
+            ("broken", lambda d: write_checkpoint(d, PRESETS["tiny"], SEED), "model.layers.1.mlp.down_proj.weight"),
+            ("broken-fp8", lambda d: write_fp8_checkpoint(d, FP8_PRESETS["tiny-fp8"], SEED),
+             "model.layers.1.mlp.down_proj.weight_scale")):
+        d = str(tmp_path / name)
+        write(d)
+        f = os.path.join(d, "model.safetensors")
+        t = load_file(f)
+        del t[missing]
+        save_file(t, f)
+        with pytest.raises(RuntimeError):
+            Engine(dict(BASE, weights=d))
 
 
 def test_checkpoint_with_its_own_tokenizer_json(tmp_path):
