@@ -253,7 +253,7 @@ ACP_DEVINL void new_token_prologue(const AttnDecodeArgs& a, const SmemLayout& L,
   const int q_dim = a.heads * HEAD_DIM, kv_dim = a.kv_heads * HEAD_DIM;
   const float* ct = a.cos_tab + (size_t)pos * (HEAD_DIM / 2);
   const float* st = a.sin_tab + (size_t)pos * (HEAD_DIM / 2);
-  const int page = a.page_table[(size_t)b * a.max_pages + pos / KV_PAGE];
+  const int page = a.page_table[a.page_off[b] + pos / KV_PAGE];
   const size_t blk = ((size_t)page * a.kv_heads + kh) * (KV_PAGE * HEAD_DIM) + (size_t)(pos % KV_PAGE) * 64;
   // rotated vectors: G query heads then the key head; 16 work items (4 frequency pairs) per head
   for (int w = tid; w < (G + 1) * 16; w += 128) {
@@ -389,7 +389,7 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
   if (warp == CONSUMER_WARPS) {
     if (lane == 0)
       produce_tiles(&tm_k, &tm_v, L.stages, L.full_bar, L.empty_bar,
-                    a.page_table + (size_t)b * a.max_pages, kh, a.kv_heads, tile_begin, tile_end, tok_end);
+                    a.page_table + a.page_off[b], kh, a.kv_heads, tile_begin, tile_end, tok_end);
     return;
   }
   const float sl2e = a.scale * 1.4426950408889634f;
@@ -442,30 +442,59 @@ attn_decode_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_consta
 
 // Finishes every (sequence, head): combines chunks x 4 warp partials in fixed order.  For a
 // single-chunk item this is the same arithmetic, in the same order, as attn_decode_item_kernel.
-__global__ void __launch_bounds__(128)
+// A 128K-token context has 512 partials per head: the max (order-free) is taken by all threads at
+// once, each partial's weight is computed once into shared memory, and the value loads of
+// MERGE_UNROLL partials are in flight together ahead of the running sums, which still add the
+// partials one by one in index order (so the bits do not depend on how the loads are batched).
+constexpr int MERGE_THREADS = 128;   // one per head dimension
+constexpr int MERGE_UNROLL = 32;
+__global__ void __launch_bounds__(MERGE_THREADS)
 attn_merge_kernel(AttnDecodeArgs a) {
+  __shared__ float s_wgt[MERGE_THREADS], s_l[MERGE_THREADS], s_max[MERGE_THREADS / 32];
   pdl_launch_dependents();
   pdl_wait();
   const int b = blockIdx.x, head = blockIdx.y, d = threadIdx.x;
   const int G = a.heads / a.kv_heads;
   const int kh = head / G, g = head % G;
-  const int n_pieces = a.chunk_cum[b + 1] - a.chunk_cum[b];
+  const int n = (a.chunk_cum[b + 1] - a.chunk_cum[b]) * CONSUMER_WARPS;   // partial i = chunk i / 4, warp i % 4
   const float sl2e = a.scale * 1.4426950408889634f;
   const size_t item = (size_t)b * a.kv_heads + kh;
-  const float* base = a.ws + ((item * a.max_chunks) * CONSUMER_WARPS * G) * 130;
+  const float* base = a.ws + ((item * a.max_chunks) * CONSUMER_WARPS * G + g) * 130;   // + i * G * 130
+  const size_t stride = (size_t)G * 130;
   float M = -INFINITY;
-  for (int p = 0; p < n_pieces; ++p)
-    for (int w = 0; w < CONSUMER_WARPS; ++w)
-      M = fmaxf(M, base[(((size_t)p * CONSUMER_WARPS + w) * G + g) * 130 + 128]);
+  for (int i = d; i < n; i += MERGE_THREADS) M = fmaxf(M, base[i * stride + 128]);
+  M = warp_max(M);
+  if ((d & 31) == 0) s_max[d >> 5] = M;
+  __syncthreads();
+  M = fmaxf(fmaxf(s_max[0], s_max[1]), fmaxf(s_max[2], s_max[3]));
   float num = 0.f, den = 0.f;
-  for (int p = 0; p < n_pieces; ++p)
-    for (int w = 0; w < CONSUMER_WARPS; ++w) {  // fixed order => deterministic
-      const float* src = base + (((size_t)p * CONSUMER_WARPS + w) * G + g) * 130;
+  for (int i0 = 0; i0 < n; i0 += MERGE_THREADS) {
+    const int cnt = min(MERGE_THREADS, n - i0);
+    if (d < cnt) {
+      const float* src = base + (i0 + d) * stride;
       const float mw = src[128];
-      const float wgt = (mw == -INFINITY) ? 0.f : exp2f((mw - M) * sl2e);
-      num += wgt * src[d];
-      den += wgt * src[129];
+      s_wgt[d] = (mw == -INFINITY) ? 0.f : exp2f((mw - M) * sl2e);
+      s_l[d] = src[129];
     }
+    __syncthreads();
+    const float* col = base + i0 * stride + d;
+    int j = 0;
+    for (; j + MERGE_UNROLL <= cnt; j += MERGE_UNROLL) {
+      float x[MERGE_UNROLL];
+#pragma unroll
+      for (int k = 0; k < MERGE_UNROLL; ++k) x[k] = col[(j + k) * stride];
+#pragma unroll
+      for (int k = 0; k < MERGE_UNROLL; ++k) {   // fixed order => deterministic
+        num += s_wgt[j + k] * x[k];
+        den += s_wgt[j + k] * s_l[j + k];
+      }
+    }
+    for (; j < cnt; ++j) {
+      num += s_wgt[j] * col[j * stride];
+      den += s_wgt[j] * s_l[j];
+    }
+    __syncthreads();
+  }
   a.out[(size_t)b * a.heads * HEAD_DIM + head * HEAD_DIM + d] = __float2bfloat16_rn(num / den);
 }
 
@@ -499,7 +528,7 @@ attn_decode_item_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_c
   if (warp == CONSUMER_WARPS) {
     if (lane == 0)
       produce_tiles(&tm_k, &tm_v, L.stages, L.full_bar, L.empty_bar,
-                    a.page_table + (size_t)b * a.max_pages, kh, a.kv_heads, 0, n_tiles, cached);
+                    a.page_table + a.page_off[b], kh, a.kv_heads, 0, n_tiles, cached);
     return;
   }
   const int r_lo = lane >> 2;
@@ -604,7 +633,7 @@ attn_prefill_kernel(const __grid_constant__ CUtensorMap tm_k, const __grid_const
   if (warp == CONSUMER_WARPS) {
     if (lane == 0)
       produce_tiles<NS>(&tm_k, &tm_v, L.stages, L.full_bar, L.empty_bar,
-                    a.page_table + (size_t)b * a.max_pages, kh, a.kv_heads, 0, n_tiles, last_pos + 1);
+                    a.page_table + a.page_off[b], kh, a.kv_heads, 0, n_tiles, last_pos + 1);
     return;
   }
   // rows of this warp: r -> token tq0 + warp*tpw + r / G, head kh*G + r % G
@@ -701,7 +730,12 @@ int launch_attn_decode(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const A
   if (a.total_chunks <= 0) return -1;
   cudaError_t e = acp_launch(attn_decode_kernel, dim3((unsigned)(a.total_chunks * a.kv_heads)), dim3(ATTN_THREADS), ATTN_SMEM, s, tm_k, tm_v, a);
   if (e != cudaSuccess) { fprintf(stderr, "[acp_infer] attn_decode launch: %s\n", cudaGetErrorString(e)); return -5; }
-  e = acp_launch(attn_merge_kernel, dim3(a.num_seqs, a.heads), dim3(128), 0, s, a);
+  return 0;
+}
+
+int launch_attn_merge(const AttnDecodeArgs& a, cudaStream_t s) {
+  if (a.num_seqs <= 0 || a.per_item) return 0;
+  cudaError_t e = acp_launch(attn_merge_kernel, dim3(a.num_seqs, a.heads), dim3(MERGE_THREADS), 0, s, a);
   if (e != cudaSuccess) { fprintf(stderr, "[acp_infer] attn_merge launch: %s\n", cudaGetErrorString(e)); return -5; }
   return 0;
 }

@@ -8,15 +8,15 @@
 namespace acp {
 
 // Decode attention.  per_item = 1: one CTA per (sequence, kv head).  Otherwise chunked: one CTA
-// per (sequence, kv head, chunk of ATTN_CHUNK_TILES x 64 tokens) + attn_merge_kernel.
+// per (sequence, kv head, chunk of ATTN_CHUNK_TILES x 64 tokens), then launch_attn_merge.
 constexpr int ATTN_CHUNK_TILES = 16;  // 1024 tokens
 struct AttnDecodeArgs {
   const __nv_bfloat16* q;   // [B][heads*128] (row b = sequence b)
   __nv_bfloat16* out;       // [B][heads*128]
   const int* ctx_len;       // [B] keys visible to the query of sequence b (incl. its own token)
   const int* chunk_cum;     // [B+1] prefix sum of the per-sequence chunk counts
-  const int* page_table;    // [B][max_pages]
-  int max_pages;
+  const int* page_table;    // packed: pages of sequence b are page_table[page_off[b] .. page_off[b+1])
+  const int* page_off;      // [B+1]
   int heads, kv_heads;
   int num_seqs;
   int total_chunks;         // chunk_cum[B]
@@ -44,8 +44,8 @@ struct AttnPrefillArgs {
   const int* q_start;       // [B] first row of the sequence's new tokens
   const int* q_len;         // [B] number of new tokens
   const int* ctx_len;       // [B] total tokens after this step (cached + new)
-  const int* page_table;
-  int max_pages;
+  const int* page_table;    // packed, as in AttnDecodeArgs
+  const int* page_off;      // [B+1]
   int heads, kv_heads;
   float scale;
 };
@@ -56,6 +56,8 @@ int attn_decode_chunks(int ctx_len);  // chunks of one sequence
 size_t attn_decode_ws_floats(int max_batch, int heads, int kv_heads, int max_chunks);
 int launch_attn_decode(const CUtensorMap& tm_k, const CUtensorMap& tm_v, const AttnDecodeArgs& a,
                        cudaStream_t s);
+// chunked decode only (no-op when per_item): combines the partials launch_attn_decode left in ws
+int launch_attn_merge(const AttnDecodeArgs& a, cudaStream_t s);
 int attn_prefill_block_tokens(int heads, int kv_heads);
 // wgmma prefill attention (attention_prefill_tc.cu): 128 query rows = 128/G tokens x G heads per CTA
 int attn_prefill_tc_setup();

@@ -118,7 +118,8 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
       const int row0 = a.q_start[b] + tq0;
       tma_load_3d(q_smem, &tm_q, &bars->q_full, 0, kh * G, row0, kEvictFirst);
       tma_load_3d(q_smem + PF_ROWS * 128, &tm_q, &bars->q_full, 64, kh * G, row0, kEvictFirst);
-      const int* pt_row = a.page_table + (size_t)b * a.max_pages;
+      const int* pt_row = a.page_table + a.page_off[b];
+      const int n_pages = a.page_off[b + 1] - a.page_off[b];
       int jk = 0, jv = 0;
       uint64_t t0 = 0;
       while (jv < n_tiles) {
@@ -129,7 +130,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
           mbar_arrive_expect_tx(&bars->k_full[s], PF_KT_BYTES);
           for (int p = 0; p < 2; ++p) {
             const int pi = jk * 2 + p;
-            const int page = pi < a.max_pages ? pt_row[pi] : 0;   // page 0 is the reserved all-zero page
+            const int page = pi < n_pages ? pt_row[pi] : 0;   // page 0 is the reserved all-zero page
             const int row = (page * a.kv_heads + kh) * 2 * KV_PAGE;
             uint8_t* dst = k_smem + s * PF_KT_BYTES + p * PF_PAGE_BYTES;
             tma_load_2d(dst, &tm_k, &bars->k_full[s], 0, row, kEvictNormal);
@@ -143,7 +144,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
           mbar_arrive_expect_tx(&bars->v_full[s], PF_KT_BYTES);
           for (int p = 0; p < 2; ++p) {
             const int pi = jv * 2 + p;
-            const int page = pi < a.max_pages ? pt_row[pi] : 0;
+            const int page = pi < n_pages ? pt_row[pi] : 0;
             const int row = (page * a.kv_heads + kh) * 2 * KV_PAGE;
             uint8_t* dst = v_smem + s * PF_KT_BYTES + p * PF_PAGE_BYTES;
             tma_load_2d(dst, &tm_v, &bars->v_full[s], 0, row, kEvictNormal);

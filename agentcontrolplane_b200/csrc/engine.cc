@@ -753,10 +753,12 @@ bool Engine::step() {
     }
     if (prefill)
       for (int t0 = 0; t0 < q; t0 += blk_tokens) { in.blk_seq[nb] = b; in.blk_tok0[nb] = t0; ++nb; }
+    // the pages that hold this step's context (Model::forward uploads these); the rest of the row is never read
     int* pt = in.page_table + (size_t)b * lim.max_pages_per_seq;
-    const int np = std::min((int)s.pages.size(), lim.max_pages_per_seq);
+    const int used = std::min((s.n_cached + q + KV_PAGE - 1) / KV_PAGE, lim.max_pages_per_seq);
+    const int np = std::min((int)s.pages.size(), used);
     for (int i = 0; i < np; ++i) pt[i] = s.pages[i];
-    for (int i = np; i < lim.max_pages_per_seq; ++i) pt[i] = 0;
+    for (int i = np; i < used; ++i) pt[i] = 0;
     if (s.n_cached + q == (int)s.tokens.size()) {  // reaches the end of known tokens: sample
       in.sample_rows[ns] = row + q - 1;
       const int gen_idx = (int)s.tokens.size() - s.prompt_len;

@@ -538,6 +538,39 @@ extern "C" size_t acp_host_splitk_workspace_bytes_fp8(int M, int K, int max_batc
   return acp::splitk_workspace_bytes_fp8(M, K, max_batch, target_ctas, strict != 0);
 }
 
+// the "model" object of acp_host_checkpoint_index and acp_host_model_preset
+static Json model_json(const acp::ModelConfig& mc) {
+  Json m = Json::object();
+  m.set("hidden", Json(mc.hidden)); m.set("layers", Json(mc.layers)); m.set("heads", Json(mc.heads));
+  m.set("kv_heads", Json(mc.kv_heads)); m.set("ffn", Json(mc.ffn)); m.set("vocab", Json(mc.vocab));
+  m.set("rope_theta", Json(mc.rope_theta)); m.set("eps", Json((double)mc.eps));
+  m.set("tied_embeddings", Json(mc.tied_embeddings)); m.set("max_pos", Json(mc.max_pos));
+  m.set("experts", Json(mc.experts));
+  if (mc.rope_factor > 0.0) {
+    Json rs = Json::array();
+    for (double v : {mc.rope_factor, mc.rope_low_freq, mc.rope_high_freq, (double)mc.rope_orig_max_pos}) rs.push(Json(v));
+    m.set("rope_scaling", rs);
+  } else {
+    m.set("rope_scaling", Json());
+  }
+  m.set("weight_dtype", Json(mc.fp8 ? "fp8_e4m3" : "bf16"));
+  float inv[64];
+  acp::rope_inv_freq(mc, inv);
+  Json fr = Json::array();
+  for (float f : inv) fr.push(Json((double)f));
+  m.set("rope_inv_freq", fr);
+  return m;
+}
+
+extern "C" int acp_host_model_preset(const char* name, char** out_json) {
+  if (!name || !out_json) return ACP_ERR_INVALID;
+  acp::ModelConfig mc;
+  if (!acp::model_preset(name, &mc)) return ACP_ERR_NOT_FOUND;
+  Json out = Json::object();
+  out.set("model", model_json(mc));
+  return ret_json(out, out_json);
+}
+
 extern "C" int acp_host_checkpoint_index(const char* path, char** out_json) {
   if (!path || !out_json) return ACP_ERR_INVALID;
   acp::Checkpoint ck;
@@ -555,18 +588,7 @@ extern "C" int acp_host_checkpoint_index(const char* path, char** out_json) {
   if (!ck.has_config()) return fail("no config.json in " + ck.dir());
   acp::ModelConfig mc;
   if (!acp::model_config_from_hf(ck.config(), &mc, &err)) return fail(err);
-  Json m = Json::object();
-  m.set("hidden", Json(mc.hidden)); m.set("layers", Json(mc.layers)); m.set("heads", Json(mc.heads));
-  m.set("kv_heads", Json(mc.kv_heads)); m.set("ffn", Json(mc.ffn)); m.set("vocab", Json(mc.vocab));
-  m.set("rope_theta", Json(mc.rope_theta)); m.set("eps", Json((double)mc.eps));
-  m.set("tied_embeddings", Json(mc.tied_embeddings)); m.set("max_pos", Json(mc.max_pos));
-  m.set("weight_dtype", Json(mc.fp8 ? "fp8_e4m3" : "bf16"));
-  float inv[64];
-  acp::rope_inv_freq(mc, inv);
-  Json fr = Json::array();
-  for (float f : inv) fr.push(Json((double)f));
-  m.set("rope_inv_freq", fr);
-  out.set("model", m);
+  out.set("model", model_json(mc));
   return ret_json(out, out_json);
 }
 

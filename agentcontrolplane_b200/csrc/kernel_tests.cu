@@ -178,9 +178,8 @@ extern "C" int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, con
   if (attn_setup_attributes() != 0) return -5;
   const int n_pages_seq = (ctx + KV_PAGE - 1) / KV_PAGE;
   const int num_pages = n_pages_seq + 3;     // page 0 reserved (all zero), two spare
-  const int max_pages = n_pages_seq + 2;
   // shuffled page table: page i of the sequence -> physical page perm[i] in 1..num_pages-1
-  std::vector<int> pt(max_pages, 0);
+  std::vector<int> pt(n_pages_seq, 0);
   for (int i = 0; i < n_pages_seq; ++i) pt[i] = 1 + (int)(((long long)i * 7 + 3) % (num_pages - 1));
   {  // make it a permutation (7 may share a factor with num_pages - 1): fall back to reversed order
     std::vector<char> seen(num_pages, 0);
@@ -211,11 +210,12 @@ extern "C" int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, con
   ACP_CUDA_CHECK(cudaMemcpy(dv.p, vc.data(), vc.size() * 2, cudaMemcpyHostToDevice));
   const int blk_tokens = impl ? attn_prefill_tc_block_tokens(heads, kv_heads) : (16 / (heads / kv_heads)) * 4;
   const int n_blocks = (q_len + blk_tokens - 1) / blk_tokens;
-  // packed ints: blk_seq[n_blocks] blk_tok0[n_blocks] q_start[1] q_len[1] ctx_len[1] page_table[max_pages]
+  // packed ints: blk_seq[n_blocks] blk_tok0[n_blocks] q_start[1] q_len[1] ctx_len[1] page_off[2] page_table[n_pages_seq]
   std::vector<int> ints;
   for (int i = 0; i < n_blocks; ++i) ints.push_back(0);
   for (int i = 0; i < n_blocks; ++i) ints.push_back(i * blk_tokens);
   ints.push_back(0); ints.push_back(q_len); ints.push_back(ctx);
+  ints.push_back(0); ints.push_back(n_pages_seq);
   for (int p : pt) ints.push_back(p);
   if (dints.alloc(ints.size() * 4)) return -5;
   ACP_CUDA_CHECK(cudaMemcpy(dints.p, ints.data(), ints.size() * 4, cudaMemcpyHostToDevice));
@@ -223,7 +223,7 @@ extern "C" int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, con
   AttnPrefillArgs pa;
   pa.q = (const __nv_bfloat16*)dq.p; pa.out = (__nv_bfloat16*)dout.p;
   pa.blk_seq = di; pa.blk_tok0 = di + n_blocks; pa.q_start = di + 2 * n_blocks; pa.q_len = di + 2 * n_blocks + 1;
-  pa.ctx_len = di + 2 * n_blocks + 2; pa.page_table = di + 2 * n_blocks + 3; pa.max_pages = max_pages;
+  pa.ctx_len = di + 2 * n_blocks + 2; pa.page_off = di + 2 * n_blocks + 3; pa.page_table = di + 2 * n_blocks + 5;
   pa.heads = heads; pa.kv_heads = kv_heads; pa.scale = 1.0f / sqrtf((float)HEAD_DIM);
   CUtensorMap tq, tk, tv;
   if (impl) {

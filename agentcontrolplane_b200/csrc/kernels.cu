@@ -182,7 +182,7 @@ int launch_add_rmsnorm(__nv_bfloat16* x, const GemmOut& add, const __nv_bfloat16
 // ---------------------------------------------------------------------------------
 __global__ void __launch_bounds__(1024)
 rope_kv_kernel(GemmOutDev qkv, const int* __restrict__ pos, const int* __restrict__ seq_of_row,
-               const int* __restrict__ page_table, int max_pages, const float* __restrict__ cos_tab,
+               const int* __restrict__ page_table, const int* __restrict__ page_off, const float* __restrict__ cos_tab,
                const float* __restrict__ sin_tab, __nv_bfloat16* __restrict__ qbuf,
                __nv_bfloat16* __restrict__ k_cache, __nv_bfloat16* __restrict__ v_cache, int heads,
                int kv_heads) {
@@ -191,7 +191,7 @@ rope_kv_kernel(GemmOutDev qkv, const int* __restrict__ pos, const int* __restric
   const int t = blockIdx.x;
   const int p = pos[t];
   const int seq = seq_of_row[t];
-  const int page = page_table[(size_t)seq * max_pages + p / KV_PAGE];
+  const int page = page_table[page_off[seq] + p / KV_PAGE];
   const int q_dim = heads * HEAD_DIM, kv_dim = kv_heads * HEAD_DIM;
   const float* ct = cos_tab + (size_t)p * (HEAD_DIM / 2);
   const float* st = sin_tab + (size_t)p * (HEAD_DIM / 2);
@@ -248,7 +248,7 @@ int launch_rope_kv(const RopeKvArgs& a, cudaStream_t s) {
   threads = ((threads + 31) / 32) * 32;
   if (threads > 1024) threads = 1024;
   ACP_LAUNCH("rope_kv", acp_launch(rope_kv_kernel, dim3(a.T), dim3(threads), 0, s, to_dev(a.qkv), a.pos,
-                                   a.seq_of_row, a.page_table, a.max_pages, a.cos_tab, a.sin_tab, a.qbuf,
+                                   a.seq_of_row, a.page_table, a.page_off, a.cos_tab, a.sin_tab, a.qbuf,
                                    a.k_cache, a.v_cache, a.heads, a.kv_heads));
   return 0;
 }

@@ -35,9 +35,9 @@ int launch_add_rmsnorm(__nv_bfloat16* x, const GemmOut& add, const __nv_bfloat16
 struct RopeKvArgs {
   GemmOut qkv;
   const int* pos;        // [T] absolute position of each row
-  const int* seq_of_row; // [T] index into page_table rows
-  const int* page_table; // [num_seqs][max_pages]
-  int max_pages;
+  const int* seq_of_row; // [T] sequence of each row
+  const int* page_table; // packed: pages of sequence b are page_table[page_off[b] .. page_off[b+1])
+  const int* page_off;   // [num_seqs+1]
   const float* cos_tab;  // [max_pos][64]
   const float* sin_tab;
   __nv_bfloat16* qbuf;   // [T][q_dim]

@@ -289,8 +289,8 @@ int Model::alloc_all() {
   ACP_TRY(dmalloc_t(allocs_, &lm_head_, (size_t)lm_rows_l_ * H));
   ACP_TRY(dmalloc_t(allocs_, &final_norm_, H));
   ACP_TRY(tma_make_weight(&m_lm_, lm_head_, lm_rows_l_, H));
-  ACP_TRY(dmalloc_t(allocs_, &cos_, (size_t)c.max_pos * 64));
-  ACP_TRY(dmalloc_t(allocs_, &sin_, (size_t)c.max_pos * 64));
+  ACP_TRY(dmalloc_t(allocs_, &cos_, (size_t)rope_rows() * 64));
+  ACP_TRY(dmalloc_t(allocs_, &sin_, (size_t)rope_rows() * 64));
   // activations (rows padded to the largest N tile, zero initialised)
   ACP_TRY(dmalloc_t(allocs_, &x_, (size_t)T * H, true));
   ACP_TRY(alloc_act(xn_, T, c.hidden, "quant_xn"));
@@ -333,11 +333,27 @@ int Model::alloc_all() {
     ACP_TRY(dmalloc_t(allocs_, &logits_gather_, (size_t)tp_size_ * lim_.max_batch * lm_rows_per_rank_));
     ACP_TRY(dmalloc_t(allocs_, &logits_full_, (size_t)lim_.max_batch * cfg_.vocab));
   }
+  // decode attention partials: every sequence may be at max_pages_per_seq pages in one step (prefix sharing lets
+  // many sequences map one long prefix), so the workspace covers max_batch x the longest context (DESIGN.md §2)
   attn_max_chunks_ = attn_decode_chunks(lim_.max_pages_per_seq * KV_PAGE);
-  ACP_TRY(dmalloc_t(allocs_, &attn_ws_, attn_decode_ws_floats(lim_.max_batch, heads_l_, kvh_l_, attn_max_chunks_)));
-  // step staging
-  ints_cap_ = (size_t)5 * lim_.max_tokens + (size_t)6 * lim_.max_batch +
-              (size_t)lim_.max_batch * lim_.max_pages_per_seq + 64;
+  const size_t attn_ws_floats = attn_decode_ws_floats(lim_.max_batch, heads_l_, kvh_l_, attn_max_chunks_);
+  {
+    size_t free_b = 0, total_b = 0;
+    ACP_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+    if (attn_ws_floats * sizeof(float) > free_b) {
+      fprintf(stderr,
+              "[acp_infer] the decode attention workspace needs %.2f GiB (max_batch %d x %d KV heads x %d chunks of 1024 "
+              "tokens at max_pages_per_seq %d) but only %.2f GiB are free beside the weights and the KV pool of %d pages: "
+              "lower max_batch, max_pages_per_seq or kv_pages\n",
+              attn_ws_floats * 4.0 / (1 << 30), lim_.max_batch, kvh_l_, attn_max_chunks_, lim_.max_pages_per_seq,
+              free_b / (double)(1 << 30), lim_.num_pages);
+      return -4;
+    }
+  }
+  ACP_TRY(dmalloc_t(allocs_, &attn_ws_, attn_ws_floats));
+  // step staging: the arrays of stage_begin, the packed page list forward() uploads, the engine's page table
+  ints_cap_ = (size_t)5 * lim_.max_tokens + (size_t)7 * lim_.max_batch +
+              (size_t)2 * lim_.max_batch * lim_.max_pages_per_seq + 72;
   ACP_TRY(dmalloc_t(allocs_, &d_ints_, ints_cap_));
   ACP_CUDA_CHECK(cudaMallocHost((void**)&h_ints_, ints_cap_ * sizeof(int)));
   ACP_TRY(dmalloc_t(allocs_, &d_sparams_, (size_t)lim_.max_batch));
@@ -393,13 +409,14 @@ int Model::gen_weights() {
   return rc;
 }
 
-// RoPE tables: same recipe as oracle/llama_oracle.py rope_tables()
+// RoPE tables: same recipe as oracle/llama_oracle.py rope_tables(), one row per position the engine can serve
 int Model::build_rope_tables() {
   const ModelConfig& c = cfg_;
-  std::vector<float> hc((size_t)c.max_pos * 64), hs((size_t)c.max_pos * 64);
+  const int rows = rope_rows();
+  std::vector<float> hc((size_t)rows * 64), hs((size_t)rows * 64);
   float inv[64];
   rope_inv_freq(c, inv);
-  for (int p = 0; p < c.max_pos; ++p)
+  for (int p = 0; p < rows; ++p)
     for (int i = 0; i < 64; ++i) {
       const float ang = (float)p * inv[i];
       hc[(size_t)p * 64 + i] = (float)cos((double)ang);
@@ -556,8 +573,12 @@ StepInput& Model::stage_begin(int T, int B, int n_blocks) {
   s.tok = carve(T); s.pos = carve(T); s.seq_of_row = carve(T);
   s.q_start = carve(B); s.q_len = carve(B); s.ctx_len = carve(B); s.sample_rows = carve(B);
   s.blk_seq = carve(n_blocks); s.blk_tok0 = carve(n_blocks);
-  s.page_table = carve((size_t)B * lim_.max_pages_per_seq);
   s.tile_cum = carve((size_t)B + 1);
+  // forward() packs the pages in use here (page offsets [B+1], then the list) and uploads up to their end;
+  // the engine's [B][max_pages_per_seq] table after them stays on the host
+  pack_at_ = off;
+  off += align4((size_t)B + 1) + align4((size_t)B * lim_.max_pages_per_seq);
+  s.page_table = carve((size_t)B * lim_.max_pages_per_seq);
   ints_used_ = off;
   s.sample_params = h_sparams_;
   return s;
@@ -669,10 +690,23 @@ int Model::forward(const StepInput& in) {
     return -1;
   }
   ACP_CUDA_CHECK(cudaSetDevice(device_));
-  // every tensor-parallel shard uploads the SAME pinned step descriptor (the lead shard's staging)
+  // every tensor-parallel shard uploads the SAME step descriptor: the lead shard's staging, copied into the shard's
+  // own pinned buffer so that each shard packs its page list without touching another's
   const int* src_ints = lead_ ? lead_->h_ints_ : h_ints_;
-  const size_t used = lead_ ? lead_->ints_used_ : ints_used_;
-  ACP_CUDA_CHECK(cudaMemcpyAsync(d_ints_, src_ints, used * sizeof(int), cudaMemcpyHostToDevice, stream_));
+  const size_t pack_at = lead_ ? lead_->pack_at_ : pack_at_;
+  if (lead_) memcpy(h_ints_, src_ints, pack_at * sizeof(int));
+  // page list: the ceil(ctx / 32) pages of each sequence, back to back; uploaded bytes follow the pages in use,
+  // not max_batch x max_pages_per_seq
+  int* h_off = h_ints_ + pack_at;
+  int* h_list = h_off + align4((size_t)in.B + 1);
+  h_off[0] = 0;
+  for (int b = 0; b < in.B; ++b) {
+    const int n = (in.ctx_len[b] + KV_PAGE - 1) / KV_PAGE;
+    memcpy(h_list + h_off[b], in.page_table + (size_t)b * lim_.max_pages_per_seq, (size_t)n * sizeof(int));
+    h_off[b + 1] = h_off[b] + n;
+  }
+  const size_t used = (size_t)(h_list - h_ints_) + (size_t)h_off[in.B];
+  ACP_CUDA_CHECK(cudaMemcpyAsync(d_ints_, h_ints_, used * sizeof(int), cudaMemcpyHostToDevice, stream_));
   h2d_bytes_ += (long long)(used * sizeof(int));
   auto dev = [&](const int* hp) { return d_ints_ + (hp - src_ints); };
   const int* d_tok = dev(in.tok);
@@ -684,7 +718,8 @@ int Model::forward(const StepInput& in) {
   const int* d_srows = dev(in.sample_rows);
   const int* d_bseq = dev(in.blk_seq);
   const int* d_btok0 = dev(in.blk_tok0);
-  const int* d_pt = dev(in.page_table);
+  const int* d_poff = d_ints_ + (h_off - h_ints_);
+  const int* d_pt = d_ints_ + (h_list - h_ints_);
   const int T = in.T;
   const float scale = 1.0f / sqrtf((float)HEAD_DIM);
 
@@ -702,7 +737,7 @@ int Model::forward(const StepInput& in) {
     if (!in.decode) {
       RopeKvArgs ra;
       ra.qkv = qkv; ra.pos = d_pos; ra.seq_of_row = d_seq; ra.page_table = d_pt;
-      ra.max_pages = lim_.max_pages_per_seq; ra.cos_tab = cos_; ra.sin_tab = sin_; ra.qbuf = qbuf_;
+      ra.page_off = d_poff; ra.cos_tab = cos_; ra.sin_tab = sin_; ra.qbuf = qbuf_;
       ra.k_cache = L.k_cache; ra.v_cache = L.v_cache; ra.T = T; ra.heads = heads_l_; ra.kv_heads = kvh_l_;
       PROF("rope_kv", launch_rope_kv(ra, stream_));
       ++launches_;
@@ -710,7 +745,7 @@ int Model::forward(const StepInput& in) {
     if (in.decode) {
       AttnDecodeArgs aa;
       aa.q = qbuf_; aa.out = attn_.x; aa.ctx_len = d_ctx; aa.chunk_cum = dev(in.tile_cum); aa.page_table = d_pt;
-      aa.max_pages = lim_.max_pages_per_seq; aa.heads = heads_l_; aa.kv_heads = kvh_l_;
+      aa.page_off = d_poff; aa.heads = heads_l_; aa.kv_heads = kvh_l_;
       aa.num_seqs = in.B;
       aa.total_chunks = in.tile_cum[in.B];   // host copy of the prefix sum (filled by the engine)
       aa.max_chunks = attn_max_chunks_;
@@ -724,11 +759,12 @@ int Model::forward(const StepInput& in) {
       if (lim_.attn_decode_mode == 1 && aa.total_chunks == in.B) aa.per_item = 1;
       if (lim_.attn_decode_mode == 2) aa.per_item = 0;
       PROF("attn_decode", launch_attn_decode(L.tm_k, L.tm_v, aa, stream_));
+      if (!aa.per_item) PROF("attn_merge", launch_attn_merge(aa, stream_));
       launches_ += aa.per_item ? 1 : 2;
     } else {
       AttnPrefillArgs pa;
       pa.q = qbuf_; pa.out = attn_.x; pa.blk_seq = d_bseq; pa.blk_tok0 = d_btok0; pa.q_start = d_qstart;
-      pa.q_len = d_qlen; pa.ctx_len = d_ctx; pa.page_table = d_pt; pa.max_pages = lim_.max_pages_per_seq;
+      pa.q_len = d_qlen; pa.ctx_len = d_ctx; pa.page_table = d_pt; pa.page_off = d_poff;
       pa.heads = heads_l_; pa.kv_heads = kvh_l_; pa.scale = scale;
       if (attn_prefill_tc_enabled()) PROF("attn_prefill", launch_attn_prefill_tc(tm_q_, L.tm_k32, L.tm_v32, pa, in.n_blocks, stream_));
       else PROF("attn_prefill", launch_attn_prefill(L.tm_k, L.tm_v, pa, in.n_blocks, stream_));

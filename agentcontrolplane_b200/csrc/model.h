@@ -5,6 +5,7 @@
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
 #include <stdint.h>
+#include <algorithm>
 #include <string>
 #include <vector>
 #include "attention.h"
@@ -48,7 +49,7 @@ struct StepInput {
   int* sample_rows; // [n_sample]
   int* blk_seq;     // [n_blocks]
   int* blk_tok0;    // [n_blocks]
-  int* page_table;  // [B][max_pages_per_seq]
+  int* page_table;  // [B][max_pages_per_seq]; entries past a sequence's ceil(ctx_len / 32) pages are not read
   int* tile_cum;    // [B+1] prefix sum of attn_decode_chunks(ctx_len) (decode attention schedule)
   SampleParams* sample_params;  // [n_sample] (pinned, separate upload when !all_greedy)
 };
@@ -93,6 +94,8 @@ class Model {
   int gen_weights();
   int load_weights(const Checkpoint& ck);   // HuggingFace Llama safetensors -> tiled/sharded HBM layout
   int build_rope_tables();
+  // positions a sequence can reach: the model's window, or less when max_pages_per_seq caps the context
+  int rope_rows() const { return std::min(cfg_.max_pos, lim_.max_pages_per_seq * KV_PAGE); }
   int choose_splits(int M, int K, int N) const;
 
   ModelConfig cfg_;
@@ -184,7 +187,8 @@ class Model {
   float* attn_ws_ = nullptr;
   int attn_max_chunks_ = 1;
   int* d_ints_ = nullptr;     // packed step ints
-  size_t ints_cap_ = 0, ints_used_ = 0;
+  size_t ints_cap_ = 0, ints_used_ = 0;   // ints_used_: carved by stage_begin
+  size_t pack_at_ = 0;        // where forward() packs the step's page offsets and page list
   int* h_ints_ = nullptr;     // pinned mirror
   SampleParams *d_sparams_ = nullptr, *h_sparams_ = nullptr;
   int *d_tokens_ = nullptr, *h_tokens_ = nullptr;

@@ -32,6 +32,15 @@ bool model_preset(const std::string& name, ModelConfig* c) {
   else if (name == "mixtral-8x7b-l2") { m.hidden = 4096; m.layers = 2; m.heads = 32; m.kv_heads = 8; m.ffn = 14336; m.experts = 8; m.rope_theta = 1000000.0; }
   else if (name == "mixtral-8x7b") { m.hidden = 4096; m.layers = 32; m.heads = 32; m.kv_heads = 8; m.ffn = 14336; m.experts = 8; m.rope_theta = 1000000.0; }
   else if (name == "llama-3-70b") { m.hidden = 8192; m.layers = 80; m.heads = 64; m.kv_heads = 8; m.ffn = 28672; }
+  // Llama-3.1: the shapes and seeded weights of the Llama-3 preset without the ".1", with the "llama3" RoPE scaling
+  // of the published checkpoints and their 131072-token window
+  else if (name == "tiny-3.1" || name == "llama-3.1-8b-l2" || name == "llama-3.1-8b") {
+    const std::string base = name == "tiny-3.1" ? "tiny" : "llama-3" + name.substr(9);
+    if (!model_preset(base, &m)) return false;
+    m.name = name;
+    m.rope_factor = 8.0; m.rope_low_freq = 1.0; m.rope_high_freq = 4.0; m.rope_orig_max_pos = 8192;
+    m.max_pos = 131072;
+  }
   else return false;
   *c = m;
   return true;
@@ -130,8 +139,7 @@ bool model_config_from_hf(const Json& hf, ModelConfig* out, std::string* err) {
   m.rope_theta = hf.get("rope_theta").as_double(10000.0);
   m.eps = (float)hf.get("rms_norm_eps").as_double(1e-5);
   m.tied_embeddings = hf.get("tie_word_embeddings").as_bool(false);
-  const int mp = (int)hf.get("max_position_embeddings").as_int(8192);
-  m.max_pos = mp < 8192 ? mp : 8192;   // table size; contexts are bounded by the KV page budget anyway
+  m.max_pos = (int)hf.get("max_position_embeddings").as_int(8192);
   const Json& rs = hf.get("rope_scaling");
   if (rs.is_object()) {
     std::string type = rs.get("rope_type").as_string();

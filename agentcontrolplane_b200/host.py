@@ -29,6 +29,7 @@ def lib():
         l.acp_host_stub_server_stop.restype = None
         l.acp_hostsim_run.argtypes = [vp, cp, out]
         l.acp_host_checkpoint_index.argtypes = [cp, out]
+        l.acp_host_model_preset.argtypes = [cp, out]
         l.acp_host_free.argtypes = [vp]
         l.acp_host_free.restype = None
         _bound = l
@@ -137,6 +138,17 @@ def checkpoint_index(path: str) -> dict:
     if rc != 0:
         raise ValueError(out.get("error", f"acp_host_checkpoint_index failed with {rc}"))
     return out
+
+
+def model_preset(name: str) -> dict:
+    """The architecture of the engine's synthetic preset `name` (the "model" object of checkpoint_index);
+    raises KeyError for a name the engine does not know."""
+    buf = ctypes.c_void_p()
+    rc = lib().acp_host_model_preset(name.encode(), ctypes.byref(buf))
+    out = json.loads(_take(buf)) if buf.value else {}
+    if rc != 0:
+        raise KeyError(name)
+    return out["model"]
 
 
 def tokenizer_encode(text: str | bytes, tokenizer_path: str | None = None) -> dict:

@@ -91,10 +91,16 @@ int acp_host_render_prompt_with(const char* tokenizer_path, const char* chat_req
  * acp_infer_init {"weights": dir} does and reports
  *   {"dir":…, "config":{…config.json…}, "tensors":{"name":{"dtype","shape","nbytes"}},
  *    "model":{"hidden":…, "layers":…, "heads":…, "kv_heads":…, "ffn":…, "vocab":…, "rope_theta":…,
- *             "eps":…, "tied_embeddings":…, "weight_dtype": "bf16" | "fp8_e4m3", "rope_inv_freq":[64 floats]}}
+ *             "eps":…, "tied_embeddings":…, "max_pos":…, "experts":…,
+ *             "rope_scaling": [factor, low_freq_factor, high_freq_factor, original_max_pos] | null,
+ *             "weight_dtype": "bf16" | "fp8_e4m3", "rope_inv_freq":[64 floats]}}
+ * max_pos is the checkpoint's max_position_embeddings (the engine serves min(max_pos, max_pages_per_seq * 32)).
  * A quantization_config other than compressed-tensors FP8_DYNAMIC (DESIGN.md §2) is refused with the field named.
  * or {"error": "..."} with return code ACP_ERR_INVALID. */
 int acp_host_checkpoint_index(const char* path, char** out_json);
+/* The synthetic preset `name` of acp_infer_init {"model": name} as {"model": {…the fields above…}};
+ * ACP_ERR_NOT_FOUND for an unknown name. */
+int acp_host_model_preset(const char* name, char** out_json);
 
 /* The engine's split-K rule for decode GEMMs (csrc/model_config.cc, pure host logic): the number of fp32 planes of
  * out[N][M] = X[N][K] W[M][K]^T, and the workspace bytes that hold the planes of ANY step of up to max_batch rows. */

@@ -53,6 +53,9 @@ typedef struct acp_engine acp_engine;
  *              tiny-g8-fp8): the same synthetic weights with the four layer projections quantised to e4m3
  *              (per-row weight scales, per-token activation scales; DESIGN.md §5); acp_infer_stats reports
  *              "weight_dtype"
+ *            | "tiny-3.1" | "llama-3.1-8b-l2" | "llama-3.1-8b" (and their -fp8 forms): the shapes and weights of
+ *              tiny / llama-3-8b-l2 / llama-3-8b with Llama-3.1's "llama3" RoPE scaling (factor 8, low 1,
+ *              high 4, original 8192) and a 131072-token window
  *   "weights": "synthetic" (seeded generator, default) | "<dir>" = HuggingFace Llama checkpoint
  *              (config.json + model.safetensors or model.safetensors.index.json + shards; BF16/F16/F32;
  *              or compressed-tensors FP8_DYNAMIC: F8_E4M3 projections with per-channel or per-tensor
@@ -60,7 +63,12 @@ typedef struct acp_engine acp_engine;
  *              "model" is then just the name requests must carry, default = the directory name)
  *   "seed": 11317760                  (0xACB200)
  *   "device": 0, "max_batch": 256, "max_tokens_per_step": 8192, "kv_pages": 2048,
- *   "max_pages_per_seq": 256, "prefix_cache": true, "tp": 1 (tensor-parallel GPUs of THIS process),
+ *   "max_pages_per_seq": 256 (KV pages of 32 tokens one sequence may hold: its context, prompt + max_tokens, is
+ *              limited to min(max_pages_per_seq * 32, the model's max_position_embeddings), beyond which a request
+ *              gets 400 context_length_exceeded; 4096 serves Llama-3.1's 131072 tokens.  Raise kv_pages with it:
+ *              the pool is shared by all sequences.  The decode attention workspace grows with
+ *              max_batch x max_pages_per_seq, DESIGN.md §2),
+ *   "prefix_cache": true, "tp": 1 (tensor-parallel GPUs of THIS process),
  *   "tp_comm": "p2p" | "nccl", "layers": n (truncated depth, dev only),
  *   "request_timeout_ms": n (0 = none): a request older than this, queued or running, ends with status 504
  *              (transient: plain error upstream => the Task is requeued, state_machine.go:757-789),
