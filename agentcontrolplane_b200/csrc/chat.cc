@@ -1,6 +1,8 @@
 // chat.cc — see chat.h.  Host-only code (no CUDA).
 #include "chat.h"
+#include <string.h>
 #include <time.h>
+#include <algorithm>
 
 namespace acp {
 
@@ -41,11 +43,6 @@ int parse_chat_request(const char* json, size_t len, ChatRequest* out, std::stri
     const Json& stop = root.get("stop");
     if ((stop.is_string() && !stop.as_string().empty()) || (stop.is_array() && stop.size() > 0)) {
       *err = "stop sequences are not supported by provider local";
-      return 400;
-    }
-    const Json& tc = root.get("tool_choice");
-    if (!tc.is_null() && !(tc.is_string() && tc.as_string() == "auto")) {
-      *err = "tool_choice other than \"auto\" is not supported by provider local";
       return 400;
     }
     if (root.get("logprobs").as_bool(false)) { *err = "logprobs are not supported by provider local"; return 400; }
@@ -105,6 +102,40 @@ int parse_chat_request(const char* json, size_t len, ChatRequest* out, std::stri
     td.parameters = fn.get("parameters");
     r.tools.push_back(std::move(td));
   }
+  // tool_choice: "auto" (or none) samples freely; "required" and a named function constrain the completion to
+  // tool calls with a grammar enforced on the GPU (grammar.h, DESIGN.md §3.3)
+  {
+    const Json& tc = root.get("tool_choice");
+    std::vector<std::string> allowed;
+    const bool constrained = !(tc.is_null() || (tc.is_string() && tc.as_string() == "auto"));
+    if (!constrained) {
+    } else if (tc.is_string() && tc.as_string() == "required") {
+      for (const ToolDef& t : r.tools) allowed.push_back(t.name);
+    } else if (tc.is_object()) {
+      const Json& fn = tc.get("function");
+      if (tc.get("type").as_string() != "function" || !fn.is_object() || !fn.get("name").is_string() ||
+          fn.get("name").as_string().empty()) {
+        *err = "tool_choice object must be {\"type\": \"function\", \"function\": {\"name\": <tool name>}}";
+        return 400;
+      }
+      const std::string name = fn.get("name").as_string();
+      bool known = false;
+      for (const ToolDef& t : r.tools) known = known || t.name == name;
+      if (!r.tools.empty() && !known) { *err = "tool_choice names function '" + name + "', which is not among the request's tools"; return 400; }
+      allowed.push_back(name);
+    } else {
+      *err = "tool_choice " + tc.dump() + " is not supported by provider local (served: \"auto\", \"required\", a named function)";
+      return 400;
+    }
+    if (constrained) {
+      if (r.tools.empty()) { *err = "tool_choice other than \"auto\" needs a non-empty tools list"; return 400; }
+      auto names = std::make_shared<GrammarNames>();
+      std::string gerr;
+      if (!build_grammar_names(allowed, names.get(), &gerr)) { *err = "tool_choice: " + gerr; return 400; }
+      r.grammar_names = std::move(names);
+      r.parallel_tool_calls = root.get("parallel_tool_calls").as_bool(true);
+    }
+  }
   SamplingParams& sp = r.sampling;
   for (const char* key : {"max_completion_tokens", "max_tokens"}) {
     const Json* mt = root.find(key);
@@ -121,6 +152,40 @@ int parse_chat_request(const char* json, size_t len, ChatRequest* out, std::stri
   if (root.find("seed") && !root.get("seed").is_null()) sp.seed = (uint64_t)root.get("seed").as_int(0);
   *out = std::move(r);
   return 0;
+}
+
+bool build_grammar_names(const std::vector<std::string>& names, GrammarNames* out, std::string* err) {
+  std::vector<std::string> esc;
+  for (const std::string& n : names) {
+    std::string e;
+    Json::escape_to(n, e);
+    Json back;
+    std::string perr;
+    if (!Json::parse(e, &back, &perr) || back.as_string() != n) { *err = "tool name is not valid UTF-8"; return false; }
+    esc.push_back(std::move(e));
+  }
+  std::sort(esc.begin(), esc.end());
+  esc.erase(std::unique(esc.begin(), esc.end()), esc.end());
+  if ((int)esc.size() > GRAMMAR_MAX_TOOLS) {
+    *err = std::to_string(esc.size()) + " tool names exceed the limit of " + std::to_string(GRAMMAR_MAX_TOOLS);
+    return false;
+  }
+  size_t total = 0;
+  for (const std::string& e : esc) total += e.size();
+  if (total > (size_t)GRAMMAR_MAX_NAME_BYTES) {
+    *err = "tool names take " + std::to_string(total) + " bytes escaped, over the limit of " + std::to_string(GRAMMAR_MAX_NAME_BYTES);
+    return false;
+  }
+  memset(out, 0, sizeof *out);
+  out->n = (int32_t)esc.size();
+  size_t at = 0;
+  for (size_t i = 0; i < esc.size(); ++i) {
+    out->off[i] = (uint16_t)at;
+    memcpy(out->bytes + at, esc[i].data(), esc[i].size());
+    at += esc[i].size();
+  }
+  out->off[esc.size()] = (uint16_t)at;
+  return true;
 }
 
 // ---------------------------------------------------------------------------------

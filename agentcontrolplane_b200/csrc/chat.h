@@ -5,8 +5,10 @@
 // written down in DESIGN.md §3 and restated for the tests in oracle/chat_oracle.py.
 #pragma once
 #include <stdint.h>
+#include <memory>
 #include <string>
 #include <vector>
+#include "grammar.h"
 #include "json.h"
 #include "tokenizer.h"
 
@@ -51,10 +53,19 @@ struct ChatRequest {
   std::vector<int> force_tokens;      // teacher-force the first generated tokens
   int return_logits = 0;              // keep fp32 logits of the first n sampled positions
   bool has_prompt_ids = false;
+  // tool_choice "required" or {"type": "function", "function": {"name": N}}: the completion is constrained to
+  // tool calls (grammar.h) of these names; null for "auto" / no tool_choice
+  std::shared_ptr<const GrammarNames> grammar_names;
+  bool parallel_tool_calls = true;    // false: exactly one call
 };
 
 // Parses an OpenAI chat-completions body.  Returns 0 or an HTTP-like 4xx status with *err set.
 int parse_chat_request(const char* json, size_t len, ChatRequest* out, std::string* err);
+
+// The grammar's name table for these tool names: each escaped as Json::escape_to writes it, sorted bytewise,
+// duplicates dropped.  False + *err when a limit (GRAMMAR_MAX_TOOLS, GRAMMAR_MAX_NAME_BYTES) is exceeded or a
+// name is not valid UTF-8 (its escaped form would not name the tool).
+bool build_grammar_names(const std::vector<std::string>& names, GrammarNames* out, std::string* err);
 
 // ---- tokenizer: see tokenizer.h; these two are the synthetic byte-level vocabulary (DESIGN.md §3.2) ----
 void encode_text(const std::string& text, std::vector<int>* ids);  // one id per UTF-8 byte

@@ -138,6 +138,25 @@ int Engine::init(const char* config_json) {
   }
   int rc = 0;
   if (tp_ == 1) {
+    // the vocabulary as bytes for tool_choice grammars (constrained requests are served on one GPU)
+    gvocab_.off.assign((size_t)mc.vocab + 1, 0);
+    gvocab_.stop.assign((size_t)mc.vocab, 0);
+    std::vector<int> one(1);
+    for (int id = 0; id < mc.vocab; ++id) {
+      if (id < tok_->vocab_size()) {
+        one[0] = id;
+        const std::string b = tok_->decode(one);
+        gvocab_.bytes.insert(gvocab_.bytes.end(), b.begin(), b.end());
+        gvocab_.stop[(size_t)id] = tok_->is_stop(id) ? 1 : 0;
+      }
+      gvocab_.off[(size_t)id + 1] = (int32_t)gvocab_.bytes.size();
+    }
+    gvocab_.view.vocab = mc.vocab;
+    gvocab_.view.off = gvocab_.off.data();
+    gvocab_.view.bytes = gvocab_.bytes.data();
+    gvocab_.view.stop = gvocab_.stop.data();
+    lim.grammar_vocab = &gvocab_.view;
+    for (int i = lim.max_batch - 1; i >= 0; --i) free_gslots_.push_back(i);
     rc = model_.init(mc, lim, device, 0, 1, nullptr, nullptr, ckpt_.get());
     if (rc != 0) return rc;
   } else {
@@ -292,6 +311,24 @@ int Engine::submit(const char* json, size_t len, uint64_t* ticket) {
       // prompt + max_tokens are reserved at admission.
       const long long left = (long long)max_ctx_tokens_ - s->prompt_len;
       s->sampling.max_tokens = (int)std::max(1LL, std::min<long long>(left, default_max_tokens_));
+    }
+    if (status == 0 && req.grammar_names) {
+      if (tp_ > 1) {
+        status = 400;
+        err = "tool_choice other than \"auto\" is served on single-GPU engines (tp = 1; use replicas), this one has tp = " +
+              std::to_string(tp_);
+      } else {
+        s->grammar_names = req.grammar_names;
+        grammar_init(&s->gstate, s->grammar_names->n, req.parallel_tool_calls);
+        GrammarState st = s->gstate;
+        for (size_t i = 0; i < req.force_tokens.size() && status == 0; ++i) {
+          if (!grammar_advance(st, *s->grammar_names, req.force_tokens[i])) {
+            status = 400;
+            err = "acp.force_tokens[" + std::to_string(i) + "] is not allowed by the tool_choice grammar";
+          }
+          if (tok_->is_stop(req.force_tokens[i])) break;
+        }
+      }
     }
     s->tools = std::move(req.tools);
     s->force_tokens = std::move(req.force_tokens);
@@ -566,9 +603,21 @@ void Engine::retain_prefix_locked(Sequence& s) {
   s.shared.clear();
 }
 
+// Advances a constrained sequence's grammar state by token `tok`; false = the grammar rejects it.
+bool Engine::grammar_advance(GrammarState& st, const GrammarNames& names, int tok) const {
+  if (tok < 0 || tok >= gvocab_.view.vocab) return false;
+  if (gvocab_.stop[(size_t)tok]) return grammar_accepting(st);
+  const int b = gvocab_.off[(size_t)tok], e = gvocab_.off[(size_t)tok + 1];
+  if (b == e) return false;
+  for (int i = b; i < e; ++i)
+    if (!grammar_step(st, gvocab_.bytes[(size_t)i], names)) return false;
+  return true;
+}
+
 void Engine::finish(const std::shared_ptr<Sequence>& s, int status, const std::string& type,
                     const std::string& msg, const std::string& finish_reason) {
   if (status == 200) retain_prefix_locked(*s); else release_pages(*s);
+  if (s->gslot >= 0) { free_gslots_.push_back(s->gslot); s->gslot = -1; }
   s->done = true;
   s->status = status;
   s->error_type = type;
@@ -656,6 +705,7 @@ void Engine::admit_locked() {
       stats_.prefix_tokens_reused += s->n_cached;
     }
     for (int i = 0; i < fresh; ++i) { s->pages.push_back(free_pages_.back()); free_pages_.pop_back(); }
+    if (s->grammar_names) { s->gslot = free_gslots_.back(); free_gslots_.pop_back(); }   // running_ < max_batch slots
     s->t_admit = clk::now();
     running_.push_back(s);
     waiting_.pop_front();
@@ -739,6 +789,7 @@ bool Engine::step() {
   int row = 0, nb = 0, ns = 0, max_ctx = 0;
   bool all_greedy = true, want_logits = false;
   std::vector<int> sample_seq;  // index into part for each sampled row
+  grows_.clear(); gup_slot_.clear(); gup_names_.clear();
   for (int b = 0; b < B; ++b) {
     Sequence& s = *part[b];
     const int q = take[b];
@@ -771,6 +822,12 @@ bool Engine::step() {
       sp.step = (uint32_t)gen_idx;
       if (s.sampling.temperature > 0.f) all_greedy = false;
       if (gen_idx < s.return_logits) want_logits = true;
+      if (s.grammar_names) {
+        GrammarRow gr;
+        gr.row = ns; gr.slot = s.gslot; gr.state = s.gstate;
+        grows_.push_back(gr);
+        if (!s.gnames_sent) { gup_slot_.push_back(s.gslot); gup_names_.push_back(s.grammar_names.get()); s.gnames_sent = true; }
+      }
       sample_seq.push_back(b);
       ++ns;
     }
@@ -782,6 +839,11 @@ bool Engine::step() {
   in.all_greedy = all_greedy;
   in.want_logits = want_logits;
   in.max_ctx = max_ctx;
+  in.n_constrained = (int)grows_.size();
+  in.g_rows = grows_.data();
+  in.n_name_uploads = (int)gup_slot_.size();
+  in.g_upload_slot = gup_slot_.data();
+  in.g_upload_names = gup_names_.data();
 
   int rc = run_forward(in);
   if (rc != 0) { fail_all_running("CUDA step failed (see stderr)"); return true; }
@@ -819,6 +881,18 @@ bool Engine::step() {
     }
     if (gen_idx < (int)s.force_tokens.size()) tok = s.force_tokens[gen_idx];
     if (gen_idx == 0) s.t_first = now;
+    if (s.grammar_names && !grammar_advance(s.gstate, *s.grammar_names, tok)) {
+      // the mask allows only tokens the grammar accepts: reaching this is an engine defect, never an answer
+      for (auto it = running_.begin(); it != running_.end(); ++it)
+        if (it->get() == &s) {
+          auto sp = *it;
+          running_.erase(it);
+          finish(sp, 500, "grammar_violation", "token " + std::to_string(tok) + " violates the tool_choice grammar", "");
+          break;
+        }
+      any_done = true;
+      continue;
+    }
     s.tokens.push_back(tok);
     const bool stop_tok = tok_->is_stop(tok);
     const bool at_cap = (gen_idx + 1 >= s.sampling.max_tokens);

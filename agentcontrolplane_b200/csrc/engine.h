@@ -37,6 +37,11 @@ struct Sequence {
   std::string error_type, error_msg, finish_reason;
   std::vector<float> logits; // return_logits x vocab
   int logits_kept = 0;
+  // tool_choice "required" / named function: the grammar's names and the state the emitted tokens reached
+  std::shared_ptr<const GrammarNames> grammar_names;
+  GrammarState gstate;
+  int gslot = -1;            // name-table slot on the device while running
+  bool gnames_sent = false;
   std::chrono::steady_clock::time_point t_submit, t_admit, t_first, t_done;
 };
 
@@ -67,6 +72,13 @@ struct EngineStats {
   std::vector<float> decode_step_ms;
 };
 
+// Every id's bytes (Tokenizer::decode({id})) and stop flag, for the grammar on the host and, once, on the device.
+struct GrammarVocabTable {
+  std::vector<int32_t> off;
+  std::vector<uint8_t> bytes, stop;
+  GrammarVocab view;
+};
+
 class Engine {
  public:
   Engine() = default;
@@ -91,12 +103,18 @@ class Engine {
   void fail_all_running(const std::string& msg);
   void release_pages(Sequence& s);
 
+  bool grammar_advance(GrammarState& st, const GrammarNames& names, int tok) const;
   int run_forward(const StepInput& in);
   void tp_worker(int idx);
 
   std::unique_ptr<Tokenizer> tok_owned_;         // "tokenizer": tokenizer.json (byte-level BPE)
   const Tokenizer* tok_ = &synthetic_tokenizer();
   std::unique_ptr<Checkpoint> ckpt_;             // "weights": <dir> — mmap'ed until the shards are loaded
+  GrammarVocabTable gvocab_;                     // tp == 1 only
+  std::vector<int> free_gslots_;
+  std::vector<GrammarRow> grows_;                // step(): the constrained rows and the name tables to upload
+  std::vector<int> gup_slot_;
+  std::vector<const GrammarNames*> gup_names_;
   Model model_;                                  // shard 0 (the only one when tp == 1)
   std::vector<std::unique_ptr<Model>> extra_;    // tensor-parallel shards 1..tp-1, one GPU each
   std::vector<NcclComm> comms_;

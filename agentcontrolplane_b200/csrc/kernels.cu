@@ -439,7 +439,7 @@ sample_kernel(const float* __restrict__ logits, int V, const SampleParams* __res
       const int bb = chosen_thread * chunk, ee = min(V, bb + chunk);
       float a2 = base;
       for (int i = bb; i < ee; ++i) {
-        if (l[i] >= lo_thr) {
+        if (l[i] >= lo_thr && l[i] > -INFINITY) {   // a masked (-inf) id is never kept, not even in the CDF's last step
           a2 += expf((l[i] - lmax) * invT);
           tok = i;  // last kept index seen; stop once the CDF passes the target
           if (a2 > target) break;

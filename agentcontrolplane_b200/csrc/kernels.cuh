@@ -3,6 +3,7 @@
 // or as `splits` fp32 partial planes [splits][n_cap][M] which it sums in index order before the
 // bf16 rounding — the deterministic split-K reduction (see gemm_wgmma.cuh).
 #pragma once
+#include "grammar.h"
 #include "model_config.h"
 #include <cuda_runtime.h>
 #include <cuda_bf16.h>
@@ -64,6 +65,11 @@ struct SampleParams {  // per row
 };
 int launch_sample(const float* logits, int V, int N, const SampleParams* params_dev,
                   int* token_out, cudaStream_t s);
+
+// Constrained decoding (grammar.cu): logits[rows[r].row][id] = -inf for every id the grammar rejects from
+// rows[r].state, name tables indexed by rows[r].slot; one grid row per constrained row (ld = row stride).
+int launch_grammar_mask(float* logits, int ld, const GrammarVocab& v, const GrammarRow* rows_dev, int n_rows,
+                        const GrammarNames* tables_dev, cudaStream_t s);
 
 // Seeded synthetic tensor (values bit-identical to oracle/synth.py).  SynthMap says where the
 // LOCAL tensor (a tensor-parallel shard, stored as contiguous 128x64 tiles, optionally with

@@ -104,6 +104,7 @@ Model::~Model() {
   if (h_sparams_) cudaFreeHost(h_sparams_);
   if (h_tokens_) cudaFreeHost(h_tokens_);
   if (h_logits_) cudaFreeHost(h_logits_);
+  if (h_grows_) cudaFreeHost(h_grows_);
   if (stream_) cudaStreamDestroy(stream_);
 }
 
@@ -361,6 +362,22 @@ int Model::alloc_all() {
   ACP_TRY(dmalloc_t(allocs_, &d_tokens_, (size_t)lim_.max_batch));
   ACP_CUDA_CHECK(cudaMallocHost((void**)&h_tokens_, lim_.max_batch * sizeof(int)));
   ACP_CUDA_CHECK(cudaMallocHost((void**)&h_logits_, (size_t)lim_.max_batch * (tp_rank_ == 0 ? cfg_.vocab : GEMM_BM) * sizeof(float)));
+  if (lim_.grammar_vocab && tp_size_ == 1) {   // constrained decoding: vocabulary bytes, name-table slots, row states
+    const GrammarVocab& v = *lim_.grammar_vocab;
+    if (v.vocab != cfg_.vocab) { fprintf(stderr, "[acp_infer] grammar vocabulary has %d ids, the model %d\n", v.vocab, cfg_.vocab); return -1; }
+    int32_t* off = nullptr;
+    uint8_t *bytes = nullptr, *stop = nullptr;
+    ACP_TRY(dmalloc_t(allocs_, &off, (size_t)v.vocab + 1));
+    ACP_TRY(dmalloc_t(allocs_, &bytes, (size_t)v.off[v.vocab]));
+    ACP_TRY(dmalloc_t(allocs_, &stop, (size_t)v.vocab));
+    ACP_CUDA_CHECK(cudaMemcpy(off, v.off, ((size_t)v.vocab + 1) * sizeof(int32_t), cudaMemcpyHostToDevice));
+    ACP_CUDA_CHECK(cudaMemcpy(bytes, v.bytes, (size_t)v.off[v.vocab], cudaMemcpyHostToDevice));
+    ACP_CUDA_CHECK(cudaMemcpy(stop, v.stop, (size_t)v.vocab, cudaMemcpyHostToDevice));
+    gvocab_.vocab = v.vocab; gvocab_.off = off; gvocab_.bytes = bytes; gvocab_.stop = stop;
+    ACP_TRY(dmalloc_t(allocs_, &d_gnames_, (size_t)lim_.max_batch));
+    ACP_TRY(dmalloc_t(allocs_, &d_grows_, (size_t)lim_.max_batch));
+    ACP_CUDA_CHECK(cudaMallocHost((void**)&h_grows_, lim_.max_batch * sizeof(GrammarRow)));
+  }
   return 0;
 }
 
@@ -826,7 +843,12 @@ int Model::forward(const StepInput& in) {
     g.tp_shard = tp_size_ > 1;
     g.w = &m_lm_.w; g.x = &m_xs_; g.M = lm_rows_l_; g.N = in.n_sample; g.K = c.hidden; g.splits = 1;
     g.epi = EPI_ARGMAX; g.ld = lm_rows_per_rank_; g.n_cap = in.n_sample;   // == lm_rows_l_ when tp == 1
-    const bool logits = in.want_logits || !in.all_greedy;
+    const bool constrained = in.n_constrained > 0;
+    if (constrained && (!d_grows_ || tp_size_ > 1 || in.n_constrained > in.n_sample)) {
+      fprintf(stderr, "[acp_infer] constrained rows on an engine that does not serve them\n");
+      return -1;
+    }
+    const bool logits = in.want_logits || !in.all_greedy || constrained;
     g.out = logits ? logits_ : nullptr;
     const float* full_logits = logits_;
     g.amax_val = amax_val_; g.amax_idx = amax_idx_;
@@ -857,9 +879,24 @@ int Model::forward(const StepInput& in) {
           ACP_TRY(launch_sample(full_logits, c.vocab, in.n_sample, d_sparams_, d_tokens_, stream_));   // greedy rows: same arg-max, lowest id
         }
       }
-    } else if (in.all_greedy) {
+    } else if (in.all_greedy && !constrained) {
       PROF("argmax_finish", launch_argmax_finish(amax_val_, amax_idx_, m_tiles, in.n_sample, d_tokens_, nullptr, stream_));
     } else {
+      if (constrained) {
+        // a sequence's name table goes up once, in its first constrained step; then only the row states
+        for (int i = 0; i < in.n_name_uploads; ++i) {
+          ACP_CUDA_CHECK(cudaMemcpyAsync(d_gnames_ + in.g_upload_slot[i], in.g_upload_names[i], sizeof(GrammarNames),
+                                         cudaMemcpyHostToDevice, stream_));
+          h2d_bytes_ += (long long)sizeof(GrammarNames);
+        }
+        memcpy(h_grows_, in.g_rows, (size_t)in.n_constrained * sizeof(GrammarRow));
+        ACP_CUDA_CHECK(cudaMemcpyAsync(d_grows_, h_grows_, (size_t)in.n_constrained * sizeof(GrammarRow),
+                                       cudaMemcpyHostToDevice, stream_));
+        h2d_bytes_ += (long long)(in.n_constrained * sizeof(GrammarRow));
+        PROF("grammar_mask", launch_grammar_mask(logits_, lm_rows_per_rank_, gvocab_, d_grows_, in.n_constrained, d_gnames_, stream_));
+        ++launches_;
+      }
+      // greedy rows of this path pick the arg-max path's token (lowest id among the maxima)
       ACP_CUDA_CHECK(cudaMemcpyAsync(d_sparams_, h_sparams_, in.n_sample * sizeof(SampleParams),
                                      cudaMemcpyHostToDevice, stream_));
       h2d_bytes_ += (long long)(in.n_sample * sizeof(SampleParams));

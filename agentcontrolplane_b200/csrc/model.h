@@ -27,6 +27,9 @@ struct ModelLimits {
   int splitk_target_ctas = 222;
   bool strict_batch_invariance = false;   // true: decode steps of > 256 rows keep the one-tile split-K factors
   int attn_decode_mode = 0;  // 0 = auto, 1 = one CTA per (sequence, kv head) when possible, 2 = always chunked + merge
+  // constrained tool-call decoding (grammar.h): every id's bytes, read once at init into a device table; null =
+  // the engine serves no constrained requests
+  const GrammarVocab* grammar_vocab = nullptr;
 };
 
 // Host-side description of one engine step (all arrays in pinned host memory, sized by limits).
@@ -52,6 +55,12 @@ struct StepInput {
   int* page_table;  // [B][max_pages_per_seq]; entries past a sequence's ceil(ctx_len / 32) pages are not read
   int* tile_cum;    // [B+1] prefix sum of attn_decode_chunks(ctx_len) (decode attention schedule)
   SampleParams* sample_params;  // [n_sample] (pinned, separate upload when !all_greedy)
+  // constrained rows (host memory of the caller): their logits are masked by the grammar before sampling
+  int n_constrained = 0;
+  const GrammarRow* g_rows = nullptr;               // [n_constrained]
+  int n_name_uploads = 0;                           // name tables to place before the mask reads them
+  const int* g_upload_slot = nullptr;               // [n_name_uploads]
+  const GrammarNames* const* g_upload_names = nullptr;
 };
 
 class Model {
@@ -193,6 +202,9 @@ class Model {
   SampleParams *d_sparams_ = nullptr, *h_sparams_ = nullptr;
   int *d_tokens_ = nullptr, *h_tokens_ = nullptr;
   float* h_logits_ = nullptr;
+  GrammarVocab gvocab_;                 // device copy of lim_.grammar_vocab
+  GrammarNames* d_gnames_ = nullptr;    // [max_batch] name tables, indexed by the engine's slot
+  GrammarRow *d_grows_ = nullptr, *h_grows_ = nullptr;   // [max_batch] the step's constrained rows
   StepInput stage_;
   std::vector<void*> allocs_;
   // per-kernel profile (ACP_PROFILE=1)

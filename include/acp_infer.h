@@ -10,7 +10,7 @@
  *
  * Wire format: the request is the SAME OpenAI chat-completions JSON body langchaingo's openai
  * provider POSTs to {baseURL}/chat/completions (model, messages[{role, content, tool_calls,
- * tool_call_id}], tools[], temperature, max_tokens, top_p, seed); the response is an OpenAI
+ * tool_call_id}], tools[], tool_choice, parallel_tool_calls, temperature, max_tokens, top_p, seed); the response is an OpenAI
  * chat.completion JSON (choices[0].message.{content | tool_calls}, usage) plus an "acp" object
  * with the emitted token ids.  Status codes follow HTTP: 200 ok, 4xx = request is invalid and
  * must not be retried (maps to llmclient.LLMRequestError, llm_client.go:18-30, which
@@ -98,7 +98,9 @@ int acp_infer_result(acp_engine* e, uint64_t ticket, char** chat_response_json, 
 
 /* fp32 logits kept for the first `acp.return_logits` sampled positions of a finished ticket
  * (parity tests).  Must be called BEFORE acp_infer_result.  Returns the number of positions
- * copied (each `vocab` floats) or a negative error. */
+ * copied (each `vocab` floats) or a negative error.  For a request constrained by tool_choice
+ * "required" or a named function these are the MASKED logits the sampler saw: -inf for every id
+ * the tool-call grammar rejects at that position (DESIGN.md §3.3). */
 int acp_infer_result_logits(acp_engine* e, uint64_t ticket, float* out, int max_positions);
 
 /* ctx.Done(): drop a queued or running request; its result reports status 499. */

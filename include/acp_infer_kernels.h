@@ -63,6 +63,20 @@ int acp_kernel_quantize_fp8(const uint16_t* x, int rows, int cols, uint8_t* code
 int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, const uint16_t* v, int heads, int kv_heads,
                             int q_len, int ctx, int impl, uint16_t* out, int iters, float* elapsed_ms);
 
+/* The tool-call grammar of tool_choice "required" / named functions (DESIGN.md §3.3) on the host, no GPU:
+ * names_json = JSON array of the allowed tool names (raw, as in `tools`), parallel = parallel_tool_calls.
+ * Runs `text` from the start state; *consumed = bytes accepted before the first rejected byte (len when none
+ * is), *complete = 1 when all of `text` was accepted and a stop token may follow. */
+int acp_kernel_grammar_accepts(const char* names_json, int parallel, const uint8_t* text, size_t len, size_t* consumed,
+                               int* complete);
+
+/* grammar_mask_kernel on the device for one row: the state `prefix` reaches (ACP_ERR_INVALID when the grammar
+ * rejects it) against a vocabulary given as byte strings — id i is vocab_bytes[vocab_off[i], vocab_off[i+1]),
+ * vocab_stop[i] != 0 marks a stop id.  allowed_bits[(vocab + 7) / 8]: bit i (LSB first) = id i allowed. */
+int acp_kernel_grammar_mask(const char* names_json, int parallel, const uint8_t* prefix, size_t prefix_len,
+                            const int32_t* vocab_off, const uint8_t* vocab_bytes, const uint8_t* vocab_stop, int vocab,
+                            uint8_t* allowed_bits);
+
 /* Number of visible CUDA devices (0 when none / no driver). */
 int acp_kernel_device_count(void);
 
