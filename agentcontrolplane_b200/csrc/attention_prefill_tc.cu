@@ -18,7 +18,9 @@
 //                O += P V_j    m64n128k16 x 4 x 2 (A = P from registers, B = V from smem, MN-major)
 //   warp 8      TMA producer: Q tile once (3-D map over qbuf [T][heads][128], box {64, G, 128/G}),
 //               then per tile K and V as four {64 dims x 32 tokens} boxes each (page x dim-half),
-//               two 2-deep rings with their own full/empty mbarriers
+//               two 2-deep rings with their own full/empty mbarriers; the V tile that holds the sequence's end
+//               lands on v_land, the warp zeroes the rows past the end (stale bytes of a recycled page), then
+//               completes v_full, so the consumers never see those bytes
 // The two warpgroups interleave on the SM: one's MMAs overlap the other's softmax.
 //
 // Reference boundary: part of the arithmetic behind langchaingo_client.go:102 (DESIGN.md §1).
@@ -70,6 +72,7 @@ ACP_DEVINL void tma_load_3d(void* smem_dst, const void* tmap, uint64_t* bar, int
 
 struct PfBars {
   uint64_t q_full;
+  uint64_t v_land;     // the sequence's last V tile landed (v_full follows once its tail is zeroed)
   uint64_t k_full[PF_STAGES], k_empty[PF_STAGES], v_full[PF_STAGES], v_empty[PF_STAGES];
 };
 
@@ -102,6 +105,7 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
     tma_prefetch_desc(&tm_k);
     tma_prefetch_desc(&tm_v);
     mbar_init(&bars->q_full, 1);
+    mbar_init(&bars->v_land, 1);
     for (int s = 0; s < PF_STAGES; ++s) {
       mbar_init(&bars->k_full[s], 1); mbar_init(&bars->k_empty[s], 8);
       mbar_init(&bars->v_full[s], 1); mbar_init(&bars->v_empty[s], 8);
@@ -141,14 +145,16 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
         }
         if (jv < jk && mbar_try_wait(&bars->v_empty[jv % PF_STAGES], (((uint32_t)(jv / PF_STAGES)) & 1u) ^ 1u)) {
           const int s = jv % PF_STAGES;
-          mbar_arrive_expect_tx(&bars->v_full[s], PF_KT_BYTES);
+          // the tile that holds the sequence's end lands on v_land: the tail below zeroes it, then fills v_full
+          uint64_t* bar = (jv * PF_KEYS + PF_KEYS > ctx) ? &bars->v_land : &bars->v_full[s];
+          mbar_arrive_expect_tx(bar, PF_KT_BYTES);
           for (int p = 0; p < 2; ++p) {
             const int pi = jv * 2 + p;
             const int page = pi < n_pages ? pt_row[pi] : 0;
             const int row = (page * a.kv_heads + kh) * 2 * KV_PAGE;
             uint8_t* dst = v_smem + s * PF_KT_BYTES + p * PF_PAGE_BYTES;
-            tma_load_2d(dst, &tm_v, &bars->v_full[s], 0, row, kEvictNormal);
-            tma_load_2d(dst + PF_HALF_BYTES, &tm_v, &bars->v_full[s], 0, row + KV_PAGE, kEvictNormal);
+            tma_load_2d(dst, &tm_v, bar, 0, row, kEvictNormal);
+            tma_load_2d(dst + PF_HALF_BYTES, &tm_v, bar, 0, row + KV_PAGE, kEvictNormal);
           }
           ++jv;
           progressed = true;
@@ -158,6 +164,24 @@ attn_prefill_tc_kernel(const __grid_constant__ CUtensorMap tm_q, const __grid_co
         else if (t0 == 0) t0 = global_timer_ns();
         else if (global_timer_ns() - t0 > 20000000000ull) __trap();
       }
+    }
+    __syncwarp();
+    const int tile0 = (n_tiles - 1) * PF_KEYS;
+    if (tile0 + PF_KEYS > ctx) {
+      // The sequence's last tile: its V rows past the end hold whatever the page's previous owner wrote there.
+      // Their P is 0, but 0 * NaN = NaN, so the producer warp zeroes them once the tile has landed, makes the
+      // stores visible to the async proxy wgmma reads shared memory through, and only then completes v_full.
+      const int s = (n_tiles - 1) % PF_STAGES;
+      mbar_wait_mma(&bars->v_land, 0);
+      uint8_t* vt = v_smem + s * PF_KT_BYTES;
+      const int first = ctx - tile0, chunks = (PF_KEYS - first) * 8;   // 16-byte chunks per dim half
+      for (int i = lane; i < 2 * chunks; i += 32) {
+        const int h = i / chunks, c = i % chunks;
+        *reinterpret_cast<uint4*>(vt + h * PF_HALF_BYTES + (first + c / 8) * 128 + (c % 8) * 16) = make_uint4(0, 0, 0, 0);
+      }
+      fence_proxy_async();
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->v_full[s]);
     }
   } else {
     // ============ consumer warpgroups: thread owns rows rb and rb + 8, keys 8c + 2(lane % 4) + {0, 1} ============

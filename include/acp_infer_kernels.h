@@ -11,7 +11,7 @@
 #define ACP_INFER_KERNELS_H
 #include <stddef.h>
 #include <stdint.h>
-/* acp_kernel_gemm / acp_kernel_gemm_fp8: a kernel stored past the end of the output */
+/* a kernel stored past the end of a hook's output, or into a K/V cache slot it does not own */
 #define ACP_ERR_GUARD (-8)
 
 #ifdef __cplusplus
@@ -62,6 +62,40 @@ int acp_kernel_quantize_fp8(const uint16_t* x, int rows, int cols, uint8_t* code
  * mma.sync kernel.  iters > 0 also times the launch (mean ms, L2 flushed between launches). */
 int acp_kernel_attn_prefill(const uint16_t* q, const uint16_t* k, const uint16_t* v, int heads, int kv_heads,
                             int q_len, int ctx, int impl, uint16_t* out, int iters, float* elapsed_ms);
+
+/* The paged K/V cache of the attention hooks below: the pages of all sequences are a shuffled permutation of
+ * physical pages 1..n (two spare), page 0 is reserved and zero, and every slot no sequence owns (the tail of a
+ * sequence's last page, the spare pages) holds the bf16 bit pattern `stale`, as a recycled page keeps its previous
+ * owner's bytes.  A kernel that changes any cache byte it does not own makes the hook return ACP_ERR_GUARD, as does
+ * a store past the end of an output buffer. */
+
+/* acp_kernel_attn_prefill for one prefill step of B sequences packed as the engine packs them: q = bf16
+ * [sum q_len][heads][128] (sequence after sequence; rows past the step hold `stale`), k, v = bf16
+ * [sum ctx_len][kv_heads][128] (each sequence's whole context), out = bf16 [sum q_len][heads][128]; query blocks per
+ * sequence as the engine builds them. */
+int acp_kernel_attn_prefill_batch(const uint16_t* q, const uint16_t* k, const uint16_t* v, int heads, int kv_heads,
+                                  int B, const int* q_len, const int* ctx_len, uint16_t stale, int impl, uint16_t* out,
+                                  int iters, float* elapsed_ms);
+
+/* One decode step of B sequences (attn_decode_item_kernel, or attn_decode_kernel + attn_merge_kernel), with the
+ * fused RoPE + K/V append of the new token.  k, v = bf16 [sum (ctx_len[b] - 1)][kv_heads][128]: positions
+ * 0..ctx_len[b]-2 of each sequence, sequence after sequence.  qkv = the QKV projection rows of the new tokens
+ * ([q heads | k heads | v heads], ld = (heads + 2 kv_heads) * 128): bf16 [B][ld] when splits = 0, else fp32 split-K
+ * planes [splits][B][ld]; the hook stores them in [n_cap] rows (n_cap >= B) whose rows B.. are NaN.  cos_tab,
+ * sin_tab = fp32 [max_pos][64].  mode 0 picks the kernel as the model does, 1 = per-item kernel (ACP_ERR_INVALID
+ * when a context needs more than one 1024-token chunk), 2 = chunked + merge.  out = bf16 [B][heads][128];
+ * k_new, v_new = bf16 [B][kv_heads][128], the cache slots of position ctx_len[b] - 1 after the step. */
+int acp_kernel_attn_decode(const uint16_t* k, const uint16_t* v, const void* qkv, int splits, int n_cap,
+                           const float* cos_tab, const float* sin_tab, int max_pos, int B, const int* ctx_len, int heads,
+                           int kv_heads, int mode, uint16_t stale, uint16_t* out, uint16_t* k_new, uint16_t* v_new);
+
+/* rope_kv_kernel over T rows of a prefill step: row t is position pos[t] of sequence seq_of_row[t] (B sequences;
+ * no (sequence, position) twice).  qkv, splits, n_cap, cos_tab, sin_tab, max_pos as for acp_kernel_attn_decode
+ * with T rows.  q_out = the rotated q rows bf16 [T][heads][128]; k_out, v_out = bf16 [T][kv_heads][128], the cache
+ * slots the rows were written to. */
+int acp_kernel_rope_kv(const void* qkv, int splits, int n_cap, int T, const int* seq_of_row, const int* pos, int B,
+                       const float* cos_tab, const float* sin_tab, int max_pos, int heads, int kv_heads, uint16_t stale,
+                       uint16_t* q_out, uint16_t* k_out, uint16_t* v_out);
 
 /* The tool-call grammar of tool_choice "required" / named functions (DESIGN.md §3.3) on the host, no GPU:
  * names_json = JSON array of the allowed tool names (raw, as in `tools`), parallel = parallel_tool_calls.
