@@ -230,7 +230,10 @@ int gemm_launch(const GemmLaunch& g, cudaStream_t stream) {
   if (g.N <= 0 || g.M <= 0) return 0;
   if (g.epi != EPI_F32 && g.splits != 1) return -1;
   if (g.fp8) return gemm_launch_e4m3(g, stream);
-  if (g.groups > 0 && (g.splits != 1 || g.group_ranges == nullptr || (g.epi != EPI_BF16 && g.epi != EPI_SWIGLU))) return -1;
+  // grouped: group g's weights are whole m-tiles g * M / 128 .. of the concatenated tensor, so M % 128 == 0
+  if (g.groups > 0 && (g.splits != 1 || g.group_ranges == nullptr || (g.epi != EPI_BF16 && g.epi != EPI_SWIGLU) ||
+                       g.groups > GEMM_GROUP_MAX || g.M % GEMM_BM || g.K % GEMM_BK))
+    return -1;
   switch (gemm_path(g)) {
     case GEMM_PATH_PERSISTENT:
       return g.epi == EPI_BF16 ? launch_persistent<EPI_BF16>(g, stream)

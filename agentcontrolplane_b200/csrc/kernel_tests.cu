@@ -6,6 +6,7 @@
 #include "gemm_wgmma.cuh"
 #include "attention.h"
 #include "fp8.h"
+#include "moe.h"
 #include <string.h>
 #include <algorithm>
 #include <utility>
@@ -538,6 +539,147 @@ extern "C" int acp_kernel_gemm_fp8(const uint8_t* w, const float* w_scale, const
   if ((rc = check_guard(dout, out_bytes)) != 0) return rc;
   ACP_CUDA_CHECK(cudaMemcpy(out, dout.p, out_bytes, cudaMemcpyDeviceToHost));
   if (iters > 0 && elapsed_ms != nullptr) return time_launches([&] { return gemm_launch(g, 0); }, iters, elapsed_ms);
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------
+// Mixture-of-experts block: the launch sequence of Model::moe_mlp on buffers sized and laid out as alloc_all and
+// load_weights make them.  xe / he / ye start as NaN, so a GEMM that reads a row the step does not own turns a
+// result NaN, and one that stores past its group leaves a changed row behind.
+// ---------------------------------------------------------------------------------
+namespace {
+// [e_local][rows][cols] row-major -> the engine's tiled layout of the concatenated experts (128 x 64 tiles,
+// [m_tile][kb]); `interleave` puts gate row j at 2j and up row j (row rows/2 + j) at 2j + 1 (gu_e_map_)
+std::vector<uint16_t> tile_experts(const uint16_t* w, int e_local, int rows, int cols, bool interleave) {
+  const int nkb = cols / GEMM_BK;
+  std::vector<uint16_t> t((size_t)e_local * rows * cols);
+  for (int e = 0; e < e_local; ++e)
+    for (int r = 0; r < rows; ++r) {
+      const int src = interleave ? (r & 1) * (rows / 2) + (r >> 1) : r;
+      const size_t g = (size_t)e * rows + r;   // row of the concatenated tensor
+      const uint16_t* s = w + ((size_t)e * rows + src) * cols;
+      for (int c = 0; c < cols; c += GEMM_BK)
+        memcpy(&t[((g / GEMM_BM) * nkb + c / GEMM_BK) * (GEMM_BM * GEMM_BK) + (g % GEMM_BM) * GEMM_BK], s + c, GEMM_BK * 2);
+    }
+  return t;
+}
+
+// rows [from, rows) of a [rows][cols] bf16 device buffer still hold the 0xffff fill
+int check_nan_rows(const DevBuf& d, size_t rows, size_t cols, size_t from, const char* what) {
+  std::vector<uint16_t> h((rows - from) * cols);
+  ACP_CUDA_CHECK(cudaMemcpy(h.data(), (const uint16_t*)d.p + from * cols, h.size() * 2, cudaMemcpyDeviceToHost));
+  for (size_t i = 0; i < h.size(); ++i)
+    if (h[i] != 0xffff) {
+      fprintf(stderr, "[acp_infer] moe: %s row %zu (past the step's %zu rows) was written\n", what, from + i / cols, from);
+      return ACP_ERR_GUARD;
+    }
+  return 0;
+}
+}  // namespace
+
+extern "C" int acp_kernel_moe(const uint16_t* xn, const uint16_t* wr, const uint16_t* wgu, const uint16_t* wdown, int T,
+                              int hidden, int ffn, int E, int e_first, int e_local, int bn, int t_cap, int partial_f32,
+                              const int32_t* topk_in, const float* topk_w_in, int32_t* topk_idx, float* topk_w,
+                              int32_t* row_of, int32_t* ranges, int32_t* tiles, int32_t* info, uint16_t* he, uint16_t* ye,
+                              void* out) {
+  if (int rc = no_device()) return rc;
+  if (!xn || !wgu || !wdown || !topk_idx || !topk_w || !row_of || !ranges || !tiles || !info || !he || !ye || !out) return -1;
+  if (T < 1 || t_cap < T || 2 * t_cap > 65535 || hidden <= 0 || ffn <= 0 || hidden % GEMM_BM || ffn % GEMM_BK) return -1;
+  if (E < 2 || E > GEMM_GROUP_MAX || e_local < 1 || e_first < 0 || e_first + e_local > E) return -1;
+  if (bn != 0 && bn != 16 && bn != 32 && bn != 64 && bn != 128 && bn != 256) return -1;
+  if ((topk_in == nullptr) != (topk_w_in == nullptr) || (topk_in == nullptr && wr == nullptr)) return -1;
+  if (topk_in)
+    for (int i = 0; i < 2 * T; ++i)
+      if (topk_in[i] < 0 || topk_in[i] >= E) return -1;
+  if (gemm_setup_attributes() != 0) return -5;
+  if (bn == 0) bn = gemm_pick_bn((2 * T + E - 1) / E);   // as Model::moe_mlp
+  const int cap = moe_tile_cap(T, bn, e_local);
+  // buffers as Model::alloc_all sizes them for max_tokens_per_step = t_cap
+  const int Tp = ((t_cap + 255) / 256) * 256;
+  const size_t rows = (size_t)2 * Tp + 256, n_ranges = (size_t)moe_ranges_ints(Tp);
+  const size_t out_bytes = (size_t)T * hidden * (partial_f32 ? 4 : 2), tk = (size_t)2 * T * 4;
+  DevBuf dxn, dwr, dgu, ddown, dxe, dhe, dye, didx, dw, drow, dranges, dout;
+  if (dxn.alloc((size_t)T * hidden * 2) || dgu.alloc((size_t)e_local * 2 * ffn * hidden * 2) ||
+      ddown.alloc((size_t)e_local * hidden * ffn * 2) || dxe.alloc(rows * hidden * 2) || dhe.alloc(rows * ffn * 2) ||
+      dye.alloc(rows * hidden * 2) || didx.alloc(tk + kGuardBytes) || dw.alloc(tk + kGuardBytes) ||
+      drow.alloc(tk + kGuardBytes) || dranges.alloc(n_ranges * 4) || dout.alloc(out_bytes + kGuardBytes))
+    return -5;
+  ACP_CUDA_CHECK(cudaMemcpy(dxn.p, xn, (size_t)T * hidden * 2, cudaMemcpyHostToDevice));
+  {
+    const std::vector<uint16_t> t = tile_experts(wgu, e_local, 2 * ffn, hidden, true);
+    ACP_CUDA_CHECK(cudaMemcpy(dgu.p, t.data(), t.size() * 2, cudaMemcpyHostToDevice));
+  }
+  {
+    const std::vector<uint16_t> t = tile_experts(wdown, e_local, hidden, ffn, false);
+    ACP_CUDA_CHECK(cudaMemcpy(ddown.p, t.data(), t.size() * 2, cudaMemcpyHostToDevice));
+  }
+  for (DevBuf* d : {&dxe, &dhe, &dye}) ACP_CUDA_CHECK(cudaMemset(d->p, 0xff, (d == &dhe ? rows * ffn : rows * hidden) * 2));
+  for (DevBuf* d : {&didx, &dw, &drow}) ACP_CUDA_CHECK(cudaMemset(d->p, 0xff, tk + kGuardBytes));
+  ACP_CUDA_CHECK(cudaMemset(dranges.p, 0xff, n_ranges * 4));
+  ACP_CUDA_CHECK(cudaMemset(dout.p, 0xff, out_bytes + kGuardBytes));
+  TmaMaps mgu, mdown, mxe, mhe;
+  if (tma_make_weight(&mgu, dgu.p, (uint64_t)e_local * 2 * ffn, hidden) || tma_make_weight(&mdown, ddown.p, (uint64_t)e_local * hidden, ffn) ||
+      tma_make_act(&mxe, dxe.p, rows, hidden) || tma_make_act(&mhe, dhe.p, rows, ffn))
+    return -5;
+  int* d_idx = (int*)didx.p;
+  float* d_w = (float*)dw.p;
+  int* d_ranges = (int*)dranges.p;
+  int rc = 0;
+  if (topk_in) {
+    ACP_CUDA_CHECK(cudaMemcpy(d_idx, topk_in, tk, cudaMemcpyHostToDevice));
+    ACP_CUDA_CHECK(cudaMemcpy(d_w, topk_w_in, tk, cudaMemcpyHostToDevice));
+  } else {
+    if (dwr.alloc((size_t)E * hidden * 2)) return -5;
+    ACP_CUDA_CHECK(cudaMemcpy(dwr.p, wr, (size_t)E * hidden * 2, cudaMemcpyHostToDevice));
+    if ((rc = launch_moe_router((const __nv_bfloat16*)dxn.p, (const __nv_bfloat16*)dwr.p, hidden, E, T, d_idx, d_w, 0))) return rc;
+  }
+  if ((rc = launch_moe_dispatch(d_idx, T, e_first, e_local, bn, d_ranges, (int*)drow.p, 0)) ||
+      (rc = launch_moe_gather((const __nv_bfloat16*)dxn.p, (const int*)drow.p, hidden, T, (__nv_bfloat16*)dxe.p, 0)))
+    return rc;
+  GemmLaunch g;
+  g.groups = e_local; g.group_ranges = d_ranges; g.splits = 1;
+  g.bn_override = bn;
+  g.N = cap * bn;
+  g.w = &mgu.w; g.x = &mxe; g.M = 2 * ffn; g.K = hidden; g.epi = EPI_SWIGLU; g.out = dhe.p; g.ld = ffn; g.n_cap = T;
+  if ((rc = gemm_launch(g, 0))) return rc;
+  g.w = &mdown.w; g.x = &mhe; g.M = hidden; g.K = ffn; g.epi = EPI_BF16; g.out = dye.p; g.ld = hidden;
+  if ((rc = gemm_launch(g, 0))) return rc;
+  if ((rc = launch_moe_combine((const __nv_bfloat16*)dye.p, (const int*)drow.p, d_w, hidden, T, dout.p, partial_f32 != 0, 0))) return rc;
+  ACP_CUDA_CHECK(cudaDeviceSynchronize());
+  for (const DevBuf* d : {&didx, &dw, &drow})
+    if ((rc = check_guard(*d, tk))) return rc;
+  if ((rc = check_guard(dout, out_bytes))) return rc;
+  std::vector<int> rg(n_ranges);
+  ACP_CUDA_CHECK(cudaMemcpy(rg.data(), d_ranges, n_ranges * 4, cudaMemcpyDeviceToHost));
+  const int n_tiles = rg[GEMM_GROUP_TILES];
+  if (n_tiles < 0 || n_tiles > cap) {
+    fprintf(stderr, "[acp_infer] moe: %d tiles, capacity %d\n", n_tiles, cap);
+    return ACP_ERR_GUARD;
+  }
+  // every int of `ranges` but the local groups, the tile count and the tile list keeps the -1 fill
+  for (size_t i = 0; i < n_ranges; ++i) {
+    const bool owned = i < (size_t)2 * e_local || i == (size_t)GEMM_GROUP_TILES ||
+                       (i >= (size_t)GEMM_GROUP_TILES + 2 && i < (size_t)GEMM_GROUP_TILES + 2 + 2 * n_tiles);
+    if (!owned && rg[i] != -1) {
+      fprintf(stderr, "[acp_infer] moe: ranges[%zu] past the tile list was written\n", i);
+      return ACP_ERR_GUARD;
+    }
+  }
+  int n_local = 0;
+  for (int e = 0; e < e_local; ++e) n_local += rg[2 * e + 1];
+  if (n_local < 0 || n_local > 2 * T) return ACP_ERR_GUARD;
+  if ((rc = check_nan_rows(dxe, rows, hidden, n_local, "xe")) || (rc = check_nan_rows(dhe, rows, ffn, n_local, "he")) ||
+      (rc = check_nan_rows(dye, rows, hidden, n_local, "ye")))
+    return rc;
+  ACP_CUDA_CHECK(cudaMemcpy(topk_idx, d_idx, tk, cudaMemcpyDeviceToHost));
+  ACP_CUDA_CHECK(cudaMemcpy(topk_w, d_w, tk, cudaMemcpyDeviceToHost));
+  ACP_CUDA_CHECK(cudaMemcpy(row_of, drow.p, tk, cudaMemcpyDeviceToHost));
+  memcpy(ranges, rg.data(), (size_t)2 * e_local * 4);
+  memcpy(tiles, rg.data() + GEMM_GROUP_TILES + 2, (size_t)2 * n_tiles * 4);
+  info[0] = bn; info[1] = n_tiles; info[2] = n_local; info[3] = cap;
+  ACP_CUDA_CHECK(cudaMemcpy(he, dhe.p, (size_t)n_local * ffn * 2, cudaMemcpyDeviceToHost));
+  ACP_CUDA_CHECK(cudaMemcpy(ye, dye.p, (size_t)n_local * hidden * 2, cudaMemcpyDeviceToHost));
+  ACP_CUDA_CHECK(cudaMemcpy(out, dout.p, out_bytes, cudaMemcpyDeviceToHost));
   return 0;
 }
 

@@ -217,12 +217,14 @@ int moe_ranges_ints(int T) { return GEMM_GROUP_TILES + 2 + 2 * (2 * T / 16 + MOE
 int moe_tile_cap(int T, int bn, int e_local) { return (2 * T + bn - 1) / bn + e_local; }
 int launch_moe_gather(const __nv_bfloat16* xn, const int* row_of, int hidden, int T, __nv_bfloat16* xe, cudaStream_t s) {
   if (T <= 0) return 0;
+  if (hidden % 8) return -1;   // 16-byte row pieces
   MOE_LAUNCH("moe_gather", acp_launch(moe_gather_kernel, dim3(T), dim3(128), 0, s, xn, row_of, hidden, xe));
   return 0;
 }
 int launch_moe_combine(const __nv_bfloat16* ye, const int* row_of, const float* topk_w, int hidden, int T, void* out,
                        bool partial_f32, cudaStream_t s) {
   if (T <= 0) return 0;
+  if (hidden % 4) return -1;   // 4 elements per thread
   if (partial_f32) MOE_LAUNCH("moe_combine_f32", acp_launch(moe_combine_kernel<true>, dim3(T), dim3(128), 0, s, ye, row_of, topk_w, hidden, out));
   else MOE_LAUNCH("moe_combine", acp_launch(moe_combine_kernel<false>, dim3(T), dim3(128), 0, s, ye, row_of, topk_w, hidden, out));
   return 0;

@@ -97,6 +97,27 @@ int acp_kernel_rope_kv(const void* qkv, int splits, int n_cap, int T, const int*
                        const float* cos_tab, const float* sin_tab, int max_pos, int heads, int kv_heads, uint16_t stale,
                        uint16_t* q_out, uint16_t* k_out, uint16_t* v_out);
 
+/* The Mixtral mixture-of-experts block of one layer, as Model::moe_mlp launches it: moe_router_kernel ->
+ * moe_dispatch_kernel -> moe_gather_kernel -> grouped gate/up GEMM with fused SwiGLU -> grouped down GEMM ->
+ * moe_combine_kernel (csrc/moe.cu, the grouped mode of csrc/gemm_wgmma.cuh).
+ *   xn = bf16 [T][hidden]; wr = bf16 [E][hidden], the router of all E experts (may be NULL with topk_in);
+ *   wgu = bf16 [e_local][2 ffn][hidden] (gate rows, then up rows) and wdown = bf16 [e_local][hidden][ffn]: the
+ *   weights of experts e_first .. e_first + e_local - 1 only, as an expert-parallel rank holds them.
+ *   bn = 0 picks the N tile of the expert GEMMs as the model does; 16, 32, 64, 128 or 256 forces one.
+ *   t_cap >= T: the max_tokens_per_step the expert buffers are sized for.
+ *   topk_in, topk_w_in = [T][2] expert ids and weights (both or neither): they replace the router's output.
+ * Outputs: topk_idx, topk_w = [T][2]; row_of = [T][2] (-1: expert not local); ranges = [e_local][2] {first row,
+ * rows}; tiles = [2 T + e_local][2], the tile list {expert, first row inside the expert}; info = {bn, tiles,
+ * n_local = local assignments, tile capacity}; he = bf16 [2 T][ffn] and ye = bf16 [2 T][hidden], of which rows
+ * 0..n_local-1 are written; out = bf16 [T][hidden], or with partial_f32 the fp32 sum over the local experts.
+ * The hook fills the expert buffers with NaN first and returns ACP_ERR_GUARD when a row past n_local of them was
+ * written, an int of the dispatch array past its tile list changed, the tile count exceeds its capacity or a store
+ * went past an output.  ACP_ERR_INVALID: hidden % 128, ffn % 64, E outside 2..16, 2 t_cap > 65535. */
+int acp_kernel_moe(const uint16_t* xn, const uint16_t* wr, const uint16_t* wgu, const uint16_t* wdown, int T, int hidden,
+                   int ffn, int E, int e_first, int e_local, int bn, int t_cap, int partial_f32, const int32_t* topk_in,
+                   const float* topk_w_in, int32_t* topk_idx, float* topk_w, int32_t* row_of, int32_t* ranges,
+                   int32_t* tiles, int32_t* info, uint16_t* he, uint16_t* ye, void* out);
+
 /* The tool-call grammar of tool_choice "required" / named functions (DESIGN.md §3.3) on the host, no GPU:
  * names_json = JSON array of the allowed tool names (raw, as in `tools`), parallel = parallel_tool_calls.
  * Runs `text` from the start state; *consumed = bytes accepted before the first rejected byte (len when none

@@ -282,35 +282,20 @@ class LlamaOracle:
             e0, e1 = the two largest logits (lowest index wins ties)
             w0, w1 = 1/(1+exp(r1-r0)), exp(r1-r0)/(1+exp(r1-r0))     (= softmax renormalised over the top 2)
             d_k    = bf16(h_k @ Wd_k^T),  h_k = bf16(bf16(silu(g)) * u),  [g|u] = bf16(xn2 @ Wgu_k^T)
-            out    = bf16(w0*d_0 + w1*d_1)     (two fp32 products, one fp32 add, one rounding)"""
+            out    = bf16(w0*d_0 + w1*d_1)     (two fp32 products, one fp32 add, one rounding)
+        The stages are the array-level functions of oracle/moe_oracle.py, which the kernel tests check one by one."""
+        from . import moe_oracle
         c = self.cfg
-        T = xn2.shape[0]
         r = router_logits(xn2, self.w.router(l))
-        e0 = np.argmax(r, axis=1)
-        r_masked = r.copy()
-        r_masked[np.arange(T), e0] = -np.inf
-        e1 = np.argmax(r_masked, axis=1)
-        ex = np.exp((r[np.arange(T), e1] - r[np.arange(T), e0]).astype(np.float32)).astype(np.float32)
-        w0 = (np.float32(1.0) / (np.float32(1.0) + ex)).astype(np.float32)
-        w1 = (ex / (np.float32(1.0) + ex)).astype(np.float32)
-        out0 = np.zeros((T, c.hidden), np.float32)
-        out1 = np.zeros((T, c.hidden), np.float32)
-        for e in range(c.experts):
-            for sel, dst in ((e0, out0), (e1, out1)):
-                rows = np.nonzero(sel == e)[0]
-                if rows.size == 0:
-                    continue
-                gu = self._r(xn2[rows] @ self.w.expert_gu(l, e).T)
-                g, u = gu[:, :c.ffn], gu[:, c.ffn:]
-                act = self._r(g / (np.float32(1.0) + np.exp(-g)))
-                dst[rows] = self._r(self._r(act * u) @ self.w.expert_down(l, e).T)
-        self.last_routing = (e0, e1, w0, w1)
+        idx, w = moe_oracle.top2(r)
+        self.last_routing = (idx[:, 0], idx[:, 1], w[:, 0], w[:, 1])
         # closest call of the discrete routing so far: gap between the 2nd and 3rd largest router logit.  bf16
         # rounding noise UPSTREAM of the router (the engine and the oracle agree on the router arithmetic bit for
         # bit, not on every bit of its input) can flip the second expert when this gap is inside that noise.
         r3 = np.partition(r, -3, axis=1)
         self.min_router_gap = min(getattr(self, "min_router_gap", np.inf), float(np.min(r3[:, -2] - r3[:, -3])))
-        return self._r((w0[:, None] * out0).astype(np.float32) + (w1[:, None] * out1).astype(np.float32))
+        return moe_oracle.moe_block(xn2, idx, w, lambda e: self.w.expert_gu(l, e), lambda e: self.w.expert_down(l, e),
+                                    c.experts, self._r)
 
     def greedy(self, prompt, max_new: int, eos=(), force=None):
         """Greedy decode; returns (token ids, per-step (top1-top2) logit margins).
